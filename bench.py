@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""bench.py -- brotli-q5 compression throughput on B200 (BASELINE.json metric), one process per GPU.
+"""bench.py -- brotli-q5 compression throughput on H100 (BASELINE.json metric), one process per GPU.
 
   python bench.py --gpus 1 --steps 5 --warmup 3
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
   python bench.py --impl reference ...      # the reference's CPU path (C restatement in oracle/) on the host cores
+  python bench.py --dump-outputs DIR ...    # also write the compressed bytes of the last timed step as DIR/<name>.npy
 
 Workload (N = 1): BASELINE.json configs[1] -- 100 MB of enwik8-shaped synthetic text, quality 5, lgwin 22.
 A step = one pass of the compression hot path over that input.  For N > 1 the stream is N x 100 MB, sharded with the
@@ -27,14 +28,15 @@ sys.path.insert(0, ROOT)
 
 WORKLOAD_BYTES = 100_000_000
 QUALITY, LGWIN = 5, 22
-# one workload string for both arms (the driver compares them): BASELINE.json configs[1]
+# one workload string for both arms, so that their lines can be compared: BASELINE.json configs[1]
 WORKLOAD = "enwik8-shaped synthetic text 100000000 bytes per GPU, quality=5, lgwin=22 (BASELINE configs[1])"
 ALG_BYTES_PER_POS_MATCH = 9  # DESIGN.md: 1 B input + 4 B sorted position read + 4 B best[] write per position
 CHUNK_BYTES = 24 << 20       # one k_match launch per chunk (csrc/bro_parse.cuh BRO_CHUNK_BYTES)
-# dram__bytes_read.sum + dram__bytes_write.sum of one k_match launch (24 MiB chunk + 4 MiB halo) from the ncu --set full
-# capture summarised in profiles/ (None until a capture of the current kernel exists)
-NCU_MATCH_DRAM_BYTES_PER_LAUNCH = 774_424_320 + 669_327_104
-NCU_MATCH_SOURCE = "profiles/r02x_ncu_q5.txt (ncu --set full, one k_match_shallow<16> launch: 29.4 M sorted entries, 25.2 M payload positions)"
+# dram__bytes_read.sum + dram__bytes_write.sum of one k_match launch (24 MiB chunk + 4 MiB halo) from an ncu --set full
+# capture on the H100 (None until a capture of the current kernel exists)
+NCU_MATCH_DRAM_BYTES_PER_LAUNCH = None
+NCU_MATCH_SOURCE = None
+DUMP_MAX_ELEMS = 4 << 20     # --dump-outputs: a larger array is written as a fixed, seeded sample of this many elements
 
 
 def load_peaks():
@@ -44,7 +46,7 @@ def load_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s; not measured)"
 
 
 class ClockSampler:
@@ -53,12 +55,13 @@ class ClockSampler:
         self.samples = []
         self.reasons = set()
         self.max_mhz = None
+        self.power_limit_w = None
         self._stop = threading.Event()
         self._t = None
 
     def _run(self):
         q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit")
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         while not self._stop.is_set():
             try:
@@ -66,6 +69,7 @@ class ClockSampler:
                                      capture_output=True, text=True, timeout=5).stdout.strip().split(",")
                 self.samples.append(float(out[0]))
                 self.max_mhz = float(out[1])
+                self.power_limit_w = float(out[6])
                 for n, v in zip(names, out[2:]):
                     if "Active" in v and "Not" not in v:
                         self.reasons.add(n)
@@ -82,7 +86,8 @@ class ClockSampler:
         if self._t:
             self._t.join(timeout=6)
         s = sorted(self.samples)
-        return {"sm_mhz": s[len(s) // 2] if s else None, "sm_max_mhz": self.max_mhz, "reasons": sorted(self.reasons)}
+        return {"sm_mhz": s[len(s) // 2] if s else None, "sm_max_mhz": self.max_mhz, "power_limit_w": self.power_limit_w,
+                "reasons": sorted(self.reasons)}
 
 
 def cpu_port_throughput(data, cores):
@@ -146,6 +151,22 @@ def run_reference(args):
     return 0
 
 
+def dump_arrays(out_dir, arrays):
+    """Writes each uint8 array as out_dir/<name>.npy in float32 (every byte value is exact), and its length as
+    out_dir/<name>_size.npy (float64).  An array longer than DUMP_MAX_ELEMS is written as the elements at a fixed, seeded
+    sample of positions (sorted; numpy default_rng(0) over its length), so that two builds that compute the same bytes
+    write the same files and the total stays below 64 MB."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a, dtype=np.uint8)
+        if a.size > DUMP_MAX_ELEMS:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_MAX_ELEMS, replace=False))
+            a = a[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float32))
+        np.save(os.path.join(out_dir, name + "_size.npy"), np.array([arrays[name].size], dtype=np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -158,7 +179,13 @@ def main():
     # "text5" = BASELINE configs[1] (the metric's configuration, the default); "json9" = BASELINE configs[3]: JSON logs, quality 9,
     # 512 MiB per GPU (4 GiB over 8 GPUs), the compress_multi split across ranks
     ap.add_argument("--config", default="text5", choices=["text5", "json9"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the compressed stream of the last resident step (compressed.npy) and of "
+                         "the last end-to-end step (stream.npy) as float32 byte values, each with its length (<name>_size.npy); "
+                         "streams longer than %d bytes are written as a fixed, seeded sample" % DUMP_MAX_ELEMS)
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.config == "json9":
         if args.bytes == WORKLOAD_BYTES:
             args.bytes = 512 << 20
@@ -323,10 +350,13 @@ def main():
     launches = 0
     ev[0].record()
     for _ in range(args.steps):
-        step_resident()
+        n_last = step_resident()
         launches += enc.timings()[1]
     ev[1].record()
     barrier()
+    dumped = {}
+    if args.dump_outputs and rank == 0:
+        dumped["compressed"] = d_out[:n_last].cpu().numpy()
     wall = ev[0].elapsed_time(ev[1]) * 1e-3
     clocks = sampler.stop()
     # ---- e2e: host buffers through the C ABI ----
@@ -338,6 +368,8 @@ def main():
         n_e2e = step_e2e()
     ev[3].record()
     barrier()
+    if args.dump_outputs and rank == 0:
+        dumped["stream"] = h_cat[:total_out if world > 1 else n_e2e].numpy().copy()
     wall_e2e = ev[2].elapsed_time(ev[3]) * 1e-3
     # the same with pageable (not pinned) host input, as a drop-in client of the C ABI would pass it
     h_pageable = torch.frombuffer(bytearray(local), dtype=torch.uint8)
@@ -395,7 +427,7 @@ def main():
                        ("synthetic JSON logs %d bytes per GPU (a 64 MB block repeated), quality=%d, lgwin=%d (BASELINE configs[3])"
                         % (NB, args.quality, LGWIN)) if args.config == "json9" else
                        "enwik8-shaped synthetic text %d bytes per GPU, quality=%d, lgwin=%d" % (NB, args.quality, LGWIN),
-                       "l2_policy": "input (100 MB) + per-position tables (>1 GB) exceed the 126 MB L2 every step",
+                       "l2_policy": "input (100 MB) + per-position tables (>1 GB) exceed the 50 MB L2 every step",
                        "pipeline": "24 MiB chunks on 4 alternating streams (lanes); H2D staging and D2H of finished output overlap compute",
                        "sharding": "compress_multi split, one shard per GPU, 4 MiB left halo, byte-aligned seams"},
             "compressed_bytes": comp_total, "ratio": round(comp_total / total_in, 5),
@@ -413,8 +445,7 @@ def main():
                          "peak_source": peak_src, "algorithmic_bytes_per_position": ALG_BYTES_PER_POS_MATCH,
                          "launch_ms": round(match_ms / max(1, -(-NB // CHUNK_BYTES)), 4),
                          "timed": "CUDA events on the launching stream, chunks serialised on one lane (K extra steps after the value loop)"},
-            # the parse has the larger share of the serialised step (profiles/r02q: 31.5 % vs 27.6 %) but is latency bound (15.8 % warps
-            # active, profiles/r02x_ncu_q5.txt), not a memory kernel
+            # the parse is latency bound (one dependent walk per parse unit), not a memory kernel
             "roofline_parse": {"kernel": "k_parse", "algorithmic_bytes_per_position": 6.8,
                                "achieved": round(6.8 * NB / (stage_acc.get("parse", 0.0) / args.steps * 1e-3) / 1e9, 1) if stage_acc.get("parse") else None,
                                "unit": "GB/s", "note": "1 B input + 4 B best[] + 12 B per command (0.15 commands / byte)"},
@@ -422,9 +453,11 @@ def main():
             "e2e": {"value": round(e2e, 1), "unit": "MB/s", "h2d_bytes_per_step": len(local), "d2h_bytes_per_step": int(total_out if rank == 0 else 0),
                     "path": "C ABI with pinned host input (H2D inside), shard outputs device-to-device over NCCL to rank 0 (exact sizes), whole stream D2H on rank 0",
                     "pageable_input_value": round(total_in * args.steps / wall_pageable / 1e6, 1)},
-            "gpu_launches": launches, "clocks": clocks,
+            "gpu_launches": launches, "device": torch.cuda.get_device_name(local_rank), "clocks": clocks,
         }
         print(json.dumps(line))
+        if args.dump_outputs:
+            dump_arrays(args.dump_outputs, dumped)
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()

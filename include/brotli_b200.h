@@ -1,4 +1,4 @@
-/* brotli_b200.h -- C ABI of the B200-native brotli compression path.
+/* brotli_b200.h -- C ABI of the GPU-native (CUDA, H100) brotli compression path.
  *
  * This library is a drop-in for the COMPRESSION entry points that the reference (dropbox/rust-brotli 8.0.4)
  * exports from its cdylib; each declaration cites the reference interface it replaces.  Decompression, the
@@ -133,7 +133,7 @@ int32_t BrotliEncoderCompressWorkPool(BrotliEncoderWorkPool* work_pool, size_t n
                                       uint8_t* encoded, size_t desired_num_threads, brotli_alloc_func alloc_func,
                                       brotli_free_func free_func, void** alloc_opaque_per_thread);
 
-/* ---- device-resident entry points (B200 additions; pointers are CUDA device pointers where noted) ---- */
+/* ---- device-resident entry points (additions of this library; pointers are CUDA device pointers where noted) ---- */
 typedef struct B200Encoder B200Encoder;
 int b200_device_count(void);
 int b200_effective_quality(int requested_quality);

@@ -1,4 +1,4 @@
-"""In-tree build of libbrotli_b200.so for sm_100a (nvcc cross-compiles without a GPU)."""
+"""In-tree build of libbrotli_b200.so for sm_90a (H100; nvcc cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
@@ -8,6 +8,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libbrotli_b200.so")
 SOURCES = ["bro_encoder.cu", "bro_capi.cu"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper); the TMA bulk copies and mbarriers need sm_90
 DEPS = ["bro_common.cuh", "bro_huffman.cuh", "bro_meta.cuh", "bro_parse.cuh", "bro_split.cuh", "bro_finalize.cuh",
         "bro_kernels.cuh", "bro_kernels_hq.cuh", "bro_hq.cuh", "bro_bsplit.cuh", "bro_encoder.h", "bro_dict.cuh", "bro_dict_data.inc"]
 
@@ -16,7 +17,8 @@ def needs_build():
     if not os.path.exists(OUT):
         return True
     t = os.path.getmtime(OUT)
-    files = [os.path.join(CSRC, f) for f in SOURCES + DEPS] + [os.path.join(ROOT, "include", "brotli_b200.h")]
+    # this file too: a library built with other flags (another architecture) is stale
+    files = [os.path.join(CSRC, f) for f in SOURCES + DEPS] + [os.path.join(ROOT, "include", "brotli_b200.h"), os.path.abspath(__file__)]
     return any(os.path.exists(f) and os.path.getmtime(f) > t for f in files)
 
 
@@ -30,7 +32,7 @@ def build(force=False, verbose=False):
     procs = []
     for f in SOURCES:
         obj = os.path.join(CSRC, f.replace(".cu", ".o"))
-        cmd = ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
+        cmd = ["nvcc"] + ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
                "-I", CSRC, "-I", os.path.join(ROOT, "include"), "-c", os.path.join(CSRC, f), "-o", obj]
         if verbose:
             cmd[1:1] = ["-Xptxas", "-v"]
@@ -39,7 +41,7 @@ def build(force=False, verbose=False):
     for p in procs:
         if p.wait() != 0:
             raise RuntimeError("nvcc failed")
-    subprocess.check_call(["nvcc", "-shared", "-o", OUT] + objs + ["-lcudart"])
+    subprocess.check_call(["nvcc"] + ARCH + ["-shared", "-o", OUT] + objs + ["-lcudart"])
     return OUT
 
 

@@ -7,7 +7,7 @@
 // BrotliHistogramRemap / BrotliHistogramReindex / BrotliClusterHistograms (cluster.rs:52-420), BrotliBuildMetaBlock
 // (metablock.rs:133-301).
 //
-// B200 re-design (what the kernels in bro_kernels_hq.cuh parallelise, and what the sequential forms below specify):
+// GPU re-design (what the kernels in bro_kernels_hq.cuh parallelise, and what the sequential forms below specify):
 //  * all costs are Q16 integers, so reductions are order independent and the CPU model equals the GPU bit for bit;
 //  * RefineEntropyCodes: sample k of the LCG sequence is seed * 16807^(k+1) mod 2^32, so the samples are independent;
 //  * FindBlocks: the symbol vector is cut into segments of BS_SEG symbols; a segment's cost vector is warmed up over the

@@ -1,4 +1,4 @@
-// bro_common.cuh -- host/device building blocks of the B200 brotli compression path.
+// bro_common.cuh -- host/device building blocks of the GPU brotli compression path.
 //
 // Everything here is a small sequential routine that runs inside ONE GPU thread (or on the host, for the
 // CPU model under tools/ that is used to check the kernels bit-for-bit).  Format constants are RFC 7932's;

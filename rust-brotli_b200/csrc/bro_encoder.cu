@@ -1,4 +1,4 @@
-// bro_encoder.cu -- host orchestration of the B200 brotli compression path and its C ABI.
+// bro_encoder.cu -- host orchestration of the GPU brotli compression path and its C ABI.
 //
 // One Encoder object = one GPU + one CUDA stream + a reusable device workspace.  A stream is compressed as a
 // sequence of independent ranges ("chunks", <= 128 MiB) whose match search sees a left halo of the previous
@@ -112,7 +112,7 @@ struct B200Encoder {
   // configuration knobs (tests flip these)
   uint32_t unit = 4096, mb_units = 1024, lcap = 64;
   int use_rle_opt = 1, split = 1, ctx_model = 1, use_dict = 1, hq_split = 1, hq_levels = HQ_MAX_LEVELS;
-  uint32_t hq_unit = 0;  // parse unit of the shortest-path parse (quality >= 10); 0 = 8 KiB at q10, 16 KiB at q11 (measured: DESIGN.md)
+  uint32_t hq_unit = 0;  // parse unit of the shortest-path parse (quality >= 10); 0 = 8 KiB at q10, 16 KiB at q11 (DESIGN.md)
   int hq_thread_units = 0;   // 1: one parse unit per thread instead of one per warp (A/B switch)
   int num_lanes = 4;
   int ondemand = 1;       // q7..q9: search deep buckets where the parse stands (1) or for every position up front (0, A/B)
@@ -133,7 +133,7 @@ struct B200Encoder {
   bool init(int dev) {
     device = dev;
     CUDA_OK(cudaSetDevice(device));
-    // (descending stream priorities per lane, to stagger the chunks, were measured: 12.1 ms vs 11.4 ms with equal priority)
+    // (descending stream priorities per lane, to stagger the chunks, were tried: slower than equal priority)
     for (auto& L : lanes) CUDA_OK(cudaStreamCreateWithFlags(&L.stream, cudaStreamNonBlocking));
     CUDA_OK(cudaStreamCreateWithFlags(&s_in, cudaStreamNonBlocking));
     CUDA_OK(cudaStreamCreateWithFlags(&s_out, cudaStreamNonBlocking));
@@ -485,9 +485,9 @@ struct B200Encoder {
     const uint32_t window = 1u << P.lgwin;
     const uint32_t payload_max = kBatchMax - window - 4096;
     // q7..q9 (bucket depth >= 64): the parse searches the buckets on demand when the chunk is a single sort batch
-    // (measured, profiles/r02u_q9_ab.log: depth >= 128 -- q8, q9 and the lgwin <= 16 configurations -- gains 1.7x..2.8x on JSON logs
-    // and periodic data and is within +-10 % on text; depth 64 (q7) and inputs of a few units are faster up front.  ondemand = 2
-    // forces the on-demand path for every deep configuration, 0 switches it off.)
+    // (depth >= 128 -- q8, q9 and the lgwin <= 16 configurations -- gains most on JSON logs and periodic data, where the walk
+    // visits few positions; depth 64 (q7) and inputs of a few units are faster up front.  ondemand = 2 forces the on-demand path
+    // for every deep configuration, 0 switches it off.)
     const bool od_shape = P.quality < 10 && (P.depth == 64 || P.depth == 128 || P.depth == 256) && range_len <= payload_max &&
                           (P.n_last == 4 || P.n_last == 10 || P.n_last == 16);
     const bool od = od_shape && (ondemand > 1 || (ondemand == 1 && P.depth >= 128 && range_len >= ((uint32_t)4 << 20)));

@@ -5,7 +5,7 @@
 // :1046-1154), UpdateNodes / EvaluateNode / StartPosQueue (hq.rs:419-821), ZopfliIterate (:1157),
 // BrotliCreateHqZopfliBackwardReferences (:1237), BrotliZopfliCreateCommands (:97).
 //
-// B200 re-design:
+// GPU re-design:
 //  * The mutating binary tree is replaced by the position-ordered bucket lists the sort stage already builds: a position's
 //    matches are the Pareto front (longer => farther) over the short-range scan, the `depth` nearest earlier positions of
 //    its bucket that share its first four bytes, and the static-dictionary candidate.  Every position is independent.
@@ -433,7 +433,7 @@ BRO_HD_NOINLINE uint32_t hq_update_nodes(const HqUnit& U, uint32_t pos, const Hq
   const uint32_t ncand = bmin((uint32_t)hq_max_candidates(U.quality), hq_queue_size(Q));
 #ifdef __CUDA_ARCH__
   // Half of the sweep's instructions were the 16 distance-cache probes per start position, almost always ending at the first-byte
-  // test (profiles/r02ag_ncu_zopfli.txt).  When the warp runs the unit in lock step, the (start k, cached distance j) pairs -- up
+  // test.  When the warp runs the unit in lock step, the (start k, cached distance j) pairs -- up
   // to 5 x 16 at quality 11 -- are spread over the lanes, three independent rounds whose loads overlap; only the pairs that can
   // improve on min_len - 1 go through the sequential part below, in the same order with the same test: identical nodes.
   uint32_t coop_len0 = 0, coop_len1 = 0, coop_len2 = 0, coop_ball0 = 0, coop_ball1 = 0, coop_ball2 = 0;
@@ -612,10 +612,10 @@ BRO_HD_NOINLINE uint32_t hq_zopfli_unit(const HqUnit& U, const HqMatch* matches,
 }
 
 // Parse unit of the shortest-path parse.  A unit is one serial node sweep, so its size is the latency of the whole stage (a 16 KiB
-// unit at quality 11 takes ~0.1 s -- more than a CPU needs for a small file), while many units are needed to fill the machine.
-// Large inputs: 8 KiB at quality 10, 16 KiB at quality 11 (size / speed trade measured in DESIGN.md); inputs known to be small get
+// unit at quality 11 takes longer than a CPU needs for a small file), while many units are needed to fill the machine.
+// Large inputs: 8 KiB at quality 10, 16 KiB at quality 11 (the size / speed trade: DESIGN.md); inputs known to be small get
 // smaller units: they cannot fill the GPU anyway, the pooled statistics (below) keep the cost model the same, and the size moves
-// by +0.05 ... +0.1 % (alice29 q11: 246 -> 33 ms).  size_hint = 0 means unknown.
+// by +0.05 ... +0.1 %.  size_hint = 0 means unknown.
 BRO_HD uint32_t hq_default_unit(int quality, uint32_t size_hint) {
   if (size_hint != 0 && size_hint <= (256u << 10)) return 2048u;
   if (size_hint != 0 && size_hint <= (1u << 20)) return 4096u;

@@ -1,4 +1,4 @@
-// bro_kernels.cuh -- CUDA kernels (sm_100a) of the brotli compression hot path.
+// bro_kernels.cuh -- CUDA kernels (sm_90a) of the brotli compression hot path.
 //
 // Stage map (DESIGN.md has the data layout and the per-kernel roofline):
 //   sort    k_sort_hist / k_scan_rows / k_scan_digits / k_sort_scatter   stable LSD radix sort of positions by
@@ -468,8 +468,8 @@ __device__ __forceinline__ void match_stage_positions(const MatchArgs& a, int64_
 }
 
 // dynamic shared memory: (MATCH_THREADS + depth) entries x 6 words.
-// Shallow buckets (depth 16 / 32: q5, q6) -- the bench path.  ncu on the loop version (profiles/r01n): 53 % of the warp
-// instructions were the divergent per-survivor loop (23 of 32 lanes active, ~11 rounds per warp).  Here every candidate
+// Shallow buckets (depth 16 / 32: q5, q6) -- the bench path.  In a loop version most of the warp instructions were the
+// divergent per-survivor loop.  Here every candidate
 // whose match is shorter than 8 bytes -- the bulk on text -- is resolved branch-free inside the unrolled scan (its length
 // comes from one XOR of the second data word), and only candidates that agree on all 8 bytes go through the exact
 // (divergent) evaluation.  Result identical to the sequential newest-first walk: highest score, nearest on ties.
@@ -562,7 +562,7 @@ __global__ void __launch_bounds__(MATCH_THREADS) k_match_shallow(MatchArgs a) {
 }
 
 // Deep buckets (depth 64..256: q7..q9 and lgwin <= 16).  With one position per lane the survivors of the 4-byte filter are
-// evaluated by 4..7 active lanes on average (ncu: 10.6 of 32 threads per instruction at q9), so here the (position,
+// evaluated by a few active lanes on average, so here the (position,
 // candidate) pairs of a whole warp are compacted and evaluated 32 at a time; results meet in a per-position atomicMax on
 // score << 16 | (255 - candidate index) << 8 | len.  "Highest score, nearest on ties" is exactly what the sequential
 // newest-first walk with strict improvement computes.  The "must be strictly longer" pre-filter uses the best of the

@@ -1,4 +1,4 @@
-// bro_kernels_hq.cuh -- CUDA kernels (sm_100a) of the quality 10 / 11 path.
+// bro_kernels_hq.cuh -- CUDA kernels (sm_90a) of the quality 10 / 11 path.
 //
 // Stage map (the specification of every stage is its sequential form in bro_hq.cuh / bro_bsplit.cuh, executed by the CPU model
 // tools/gpu_model.cpp; the kernels must reproduce it bit for bit):

@@ -3,7 +3,7 @@
 // Reference semantics: store_meta_block (brotli_bit_stream.rs:2035-2261) with its helpers
 // StoreCompressedMetaBlockHeader :1292, BuildAndStoreBlockSplitCode :1536, StoreBlockSwitch :1506,
 // StoreTrivialContextMap :1613, EncodeContextMap :1783, StoreCommandExtra :1947.
-// B200 re-design: the header of a metablock is produced by one thread into a private scratch buffer; the
+// GPU re-design: the header of a metablock is produced by one thread into a private scratch buffer; the
 // body is emitted by one thread per command at a bit offset obtained from a prefix sum of exact bit
 // lengths (the same routine is instantiated with a counting writer and with an atomic-OR writer).
 #pragma once

@@ -1,7 +1,7 @@
 // bro_parse.cuh -- match scoring and the greedy+lazy parse of one parse unit (one GPU thread per unit).
 //
 // Reference semantics: FindLongestMatch scoring (backward_references/mod.rs:1871-1889, 1151-1154; H9 :657-708)
-// and CreateBackwardReferences (mod.rs:2376-2552).  B200 re-design: the hash-bucket walk is NOT done here --
+// and CreateBackwardReferences (mod.rs:2376-2552).  GPU re-design: the hash-bucket walk is NOT done here --
 // the match kernel has already produced, for every position, the best bucket candidate (best[p] =
 // distance << 8 | min(len, LCAP)) in parallel; the serial part left is the last-distance probes, lazy
 // deferral, and command emission, over a unit of a few KiB with a unit-local distance cache.
@@ -15,8 +15,8 @@ namespace bro {
 
 // length of the chunk that starts `done` bytes into a range of `total` bytes (shared by the encoder and its CPU model)
 BRO_HD uint32_t chunk_len_at(uint64_t done, uint64_t total) {
-  // (a short first chunk, to start computing before the whole first 24 MiB are staged, was measured: e2e unchanged,
-  // HBM-resident throughput -5 % because the last chunk then no longer hides behind the others)
+  // (a short first chunk, to start computing before the whole first 24 MiB are staged, does not pay: e2e gains nothing and
+  // the HBM-resident throughput drops because the last chunk then no longer hides behind the others)
   const uint64_t left = total - done;
   return (uint32_t)(left < BRO_CHUNK_BYTES ? left : BRO_CHUNK_BYTES);
 }

@@ -1,4 +1,4 @@
-//! Drop-in surface of the reference crate's compression path on top of libbrotli_b200 (CUDA, sm_100a).
+//! Drop-in surface of the reference crate's compression path on top of libbrotli_b200 (CUDA, sm_90a).
 //!
 //! Same names and argument meaning as the reference:
 //!   * `BrotliEncoderParams`                 src/enc/backward_references/mod.rs:71, defaults src/enc/encode.rs:318-357
@@ -79,7 +79,7 @@ impl Stream {
         let s = Stream { h };
         for (k, v) in params.key_values() {
             if unsafe { ffi::BrotliEncoderSetParameter(s.h, k, v) } == 0 {
-                return Err(io::Error::new(ErrorKind::InvalidInput, "parameter not produced by the B200 path"));
+                return Err(io::Error::new(ErrorKind::InvalidInput, "parameter not produced by the GPU path"));
             }
         }
         Ok(s)

@@ -1,14 +1,18 @@
 """Regenerates tests/golden/: copies the reference's small test inputs (public test vectors, not source code) and
 records, for each (file, quality, lgwin): the size produced by the C restatement in oracle/ (with sha256 of its
 stream), the size produced by Google's libbrotlienc 1.1.0 (the code the reference was ported from), and the size +
-sha256 of the CPU model of the GPU pipeline.  Run in the development container (needs /root/reference)."""
+sha256 of the CPU model of the GPU pipeline.
+
+  python tests/golden/make_golden.py [TESTDATA_DIR]
+
+TESTDATA_DIR is the reference's testdata/ directory to copy the inputs from; without it the inputs already stored here are
+used and only golden_sizes.json is rewritten."""
 import hashlib, json, os, shutil, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 from oracle.harness import Oracle, sys_compress, sys_decompress
 from tools.model_harness import Model
 
-SRC = "/root/reference/testdata"
 FILES = ["alice29.txt", "asyoulik.txt", "random_then_unicode", "quickfox_repeated", "random_org_10k.bin", "backward65536",
          "64x", "ukkonooa", "monkey", "x", "xyzzy", "10x10y", "aaabaaaa", "empty", "quickfox", "compressed_file"]
 CONFIGS = [(5, 20), (5, 22), (6, 22), (7, 22), (8, 22), (9, 22), (9, 16), (5, 24), (5, 18), (10, 22), (11, 22), (11, 24), (10, 16)]
@@ -16,12 +20,13 @@ CONFIGS = [(5, 20), (5, 22), (6, 22), (7, 22), (8, 22), (9, 22), (9, 16), (5, 24
 # the reference was ported from: alice29 q10 = 47 477 B, q11 = 46 487 B against the reference's own KATs 47 488 / 46 493,
 # src/bin/integration_tests.rs:408-449) -- "oracle_size" then holds that size and "size_reference" says so.
 
-def main():
+def main(src=None):
     here = os.path.dirname(os.path.abspath(__file__))
     o, m = Oracle(), Model()
     table = {}
     for f in FILES:
-        shutil.copyfile(os.path.join(SRC, f), os.path.join(here, f))
+        if src:
+            shutil.copyfile(os.path.join(src, f), os.path.join(here, f))
         d = open(os.path.join(here, f), "rb").read()
         for q, w in CONFIGS:
             sc = sys_compress(d, q, w)
@@ -44,4 +49,4 @@ def main():
     print("wrote", len(table), "entries")
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1] if len(sys.argv) > 1 else None)

@@ -1,6 +1,6 @@
 """Deterministic synthetic inputs for the BASELINE.json configs (SURVEY.md section 8d).
 
-Nothing here reads /root/reference: the GPU box does not have it.  All generators are seeded and vectorised
+Nothing here reads files outside the repository.  All generators are seeded and vectorised
 with numpy so that 100 MB takes seconds.
 
   enwik_like(n, seed=8)   -- Wikipedia-XML-shaped UTF-8 text: Zipfian pseudo-word vocabulary driven by an
