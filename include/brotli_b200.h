@@ -155,6 +155,11 @@ int b200_encoder_compress_range(B200Encoder* e, int quality, int lgwin, uint64_t
 int b200_encoder_last_timings(B200Encoder* e, float* ms, uint32_t* launches);
 /* stage hook used by the parity tests: per-position best bucket match (distance << 8 | capped length) */
 int b200_stage_match(B200Encoder* e, int quality, int lgwin, const uint8_t* in, size_t n, uint32_t* best_out);
+/* stage hook of quality 10 / 11 (n <= one chunk): matches per position hqn[n], hqm[n][16][2] (distance, length word); per parse
+ * unit ncmd, tail, ncopy as units[3][nu]; raw commands raw[nu][unit / 2 + 1][3].  b200_hq_unit gives the unit for size_hint n. */
+int b200_stage_hq(B200Encoder* e, int quality, int lgwin, const uint8_t* in, size_t n, uint8_t* hqn, uint32_t* hqm, uint32_t* units,
+                  uint32_t* raw);
+uint32_t b200_hq_unit(B200Encoder* e, int quality, uint64_t size_hint);
 
 #ifdef __cplusplus
 }

@@ -40,6 +40,10 @@ def lib():
         L.b200_encoder_last_timings.argtypes = [vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_uint32)]
         L.b200_stage_match.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp, sz, vp]
         L.b200_stage_match.restype = ctypes.c_int
+        L.b200_stage_hq.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp, sz, vp, vp, vp, vp]
+        L.b200_stage_hq.restype = ctypes.c_int
+        L.b200_hq_unit.argtypes = [vp, ctypes.c_int, ctypes.c_uint64]
+        L.b200_hq_unit.restype = ctypes.c_uint32
         _lib = L
     return _lib
 
@@ -118,3 +122,22 @@ class DeviceEncoder:
         if not ok:
             raise RuntimeError("b200_stage_match failed")
         return out
+
+    def stage_hq(self, data: bytes, quality: int, lgwin: int):
+        """Quality 10 / 11 stage results of one chunk: (hqn[n] u8, hqm[n][16][2] u32 (dist, lc), units[3][nu] u32 (ncmd, tail,
+        ncopy), raw[nu][unit/2+1][3] u32, unit).  hqm entries past hqn[p] are left over from earlier calls."""
+        import numpy as np
+        n = len(data)
+        unit = int(self._L.b200_hq_unit(self._h, quality, n))
+        if n == 0 or unit == 0:
+            raise ValueError("stage_hq needs quality >= 10 and a non-empty input")
+        nu = (n + unit - 1) // unit
+        hqn = np.zeros(n, dtype=np.uint8)
+        hqm = np.zeros((n, 16, 2), dtype=np.uint32)
+        units = np.zeros((3, nu), dtype=np.uint32)
+        raw = np.zeros((nu, unit // 2 + 1, 3), dtype=np.uint32)
+        ok = self._L.b200_stage_hq(self._h, quality, lgwin, _inptr(data), n, hqn.ctypes.data, hqm.ctypes.data, units.ctypes.data,
+                                   raw.ctypes.data)
+        if not ok:
+            raise RuntimeError("b200_stage_hq failed")
+        return hqn, hqm, units, raw, unit

@@ -877,4 +877,12 @@ int b200_stage_hq(B200Encoder* e, int quality, int lgwin, const uint8_t* in, siz
   return ok ? 1 : 0;
 }
 
+// parse unit the quality >= 10 path uses for this size hint with the encoder's current options (sizes the b200_stage_hq buffers)
+uint32_t b200_hq_unit(B200Encoder* e, int quality, uint64_t size_hint) {
+  if (!e || quality < 10) return 0;
+  EncParams P;
+  e->fill_params(&P, quality, 22, size_hint);
+  return P.unit;
+}
+
 }  // extern "C"

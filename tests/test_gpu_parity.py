@@ -107,13 +107,18 @@ def test_edge_sizes(encoder, model, n):
 
 @pytest.mark.parametrize("q", [9, 10, 11])
 def test_edge_sizes_deep_and_hq(encoder, model, q):
-    """The sizes that switch something on in the q9 on-demand search (forced) and in the q10 / q11 path: first bucket match, the
-    long-prefix levels (8 + 8 / 16 / 32 bytes), the 512-byte warm-up, 8 / 16 KiB parse units, the 64 KiB statistics window."""
+    """The sizes that switch something on in the q9 on-demand search (forced; 4 KiB parse units) and in the q10 / q11 path with
+    its default unit for inputs up to 256 KiB (2 KiB): first bucket match, the long-prefix levels (8 + 8 / 16 / 32 bytes), one
+    and two units, the 512-byte warm-up behind a unit seam, the 64 KiB statistics window.  The other unit sizes:
+    test_gpu_hq.py."""
     import rust_brotli_b200 as rb
     src = golden_bytes("alice29.txt") * 2
+    sizes = [0, 1, 2, 3, 7, 8, 9, 39, 40, 41, 63, 64, 65, 511, 512, 513, 4097, 8191, 8192, 8193, 16383, 16385, 65535, 65536,
+             65537, 70001, 131073]
+    sizes += [4095, 4096, 4607, 4608, 4609] if q == 9 else [2047, 2048, 2049, 2559, 2560, 2561]
     encoder.set_option(rb._native.OPT_ONDEMAND, 2)
     try:
-        for n in (0, 1, 2, 3, 7, 8, 9, 39, 40, 41, 63, 64, 65, 511, 512, 513, 4097, 8191, 8192, 8193, 16383, 16385, 65535, 65537, 70001):
+        for n in sizes:
             d = src[:n]
             c = encoder.compress(d, q, 22)
             assert sys_decompress(c, max(n, 1)) == d, n

@@ -185,10 +185,31 @@ def test_catable_framing_stitches_like_brocatli(model, q):
 
 
 @pytest.mark.parametrize("q", [10, 11])
+def test_model_hq_matches_equal_brute_force(model, q):
+    """The all-matches stage of quality 10 / 11 against tests/hq_ref.py, a numpy restatement of its contract (short distances,
+    256-deep 4-byte buckets, 1024-deep 8 / 16 / 32-byte levels, Pareto fronts of the 8 longest): every window entry of every
+    position must agree.  Inputs: planted copies at the distance / length edges, text and JSON logs, and a two-byte period that
+    fills every bucket to its depth."""
+    import hq_ref
+    from tools import datagen
+    alice = golden_bytes("alice29.txt")
+    cases = [(hq_ref.planted_input(10), 10), (hq_ref.planted_input(16), 16), (alice[:60000], 16), (alice[:30000], 12),
+             (datagen.json_logs(40000), 12 if q == 10 else 16), (b"ab" * 6000, 10), (b"ab" * 6000 + alice[:3000], 16)]
+    for d, w in cases:
+        cnt, ent = hq_ref.hq_ref(d, q, w)
+        hqn, hqm, _, _, _ = model.stage_hq(d, q, w)
+        got = hq_ref.window_part(hqn, hqm)
+        diff = hq_ref.first_difference(cnt, ent, *got)
+        assert diff is None, "n=%d lgwin=%d: %s" % (len(d), w, diff)
+        assert cnt.sum() > 10000  # the inputs are full of matches: the comparison is not vacuous
+
+
+@pytest.mark.parametrize("q", [10, 11])
 @pytest.mark.parametrize("n", [0, 1, 2, 3, 7, 8, 9, 39, 40, 41, 63, 64, 65, 511, 512, 513, 8191, 8192, 8193, 16383, 16385, 70001])
 def test_model_hq_edge_sizes(model, q, n):
     """quality 10 / 11 around every size that switches something on: 8 bytes (first bucket match), 8 + 8 / 16 / 32 bytes (the
-    long-prefix levels), the 512-byte warm-up, the 8 / 16 KiB parse units, the 64 KiB statistics window."""
+    long-prefix levels), the 512-byte warm-up, one and more 2 KiB parse units (the default up to 256 KiB), the 64 KiB
+    statistics window."""
     d = (golden_bytes("alice29.txt") * 2)[:n]
     c, _ = model.compress(d, q, 22)
     assert sys_decompress(c, max(n, 1)) == d

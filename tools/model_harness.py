@@ -31,6 +31,7 @@ class Model:
         self.lib.gpu_model_compress.argtypes = [ctypes.POINTER(EncParams), ctypes.c_char_p, ctypes.c_char_p, ctypes.c_size_t,
                                                 ctypes.POINTER(ModelStats), ctypes.c_void_p]
         self.lib.gpu_model_default_params.argtypes = [ctypes.POINTER(EncParams), ctypes.c_int, ctypes.c_int, ctypes.c_uint32, ctypes.c_uint32]
+        self.lib.gpu_model_debug_hq.argtypes = [ctypes.c_void_p] * 4
     def params(self, q, lgwin, n, size_hint=0, **kw):
         p = EncParams()
         self.lib.gpu_model_default_params(ctypes.byref(p), q, lgwin, n, size_hint)
@@ -57,3 +58,25 @@ class Model:
         n = self.lib.gpu_model_compress(ctypes.byref(p), data, out, cap, ctypes.byref(st), best_out)
         if n == 0: raise RuntimeError("model failed")
         return out.raw[:n], st
+
+    def stage_hq(self, data, q, lgwin, **kw):
+        """Quality 10 / 11 stage results of a one-chunk input, laid out as DeviceEncoder.stage_hq returns them:
+        (hqn, hqm, units, raw, unit)."""
+        import numpy as np
+        n = len(data)
+        if not 0 < n <= 24 << 20 or q < 10:
+            raise ValueError("stage_hq covers one chunk (1 .. 24 MiB) at quality >= 10")
+        unit = self.params(q, lgwin, n, 0, **kw).unit
+        nu = (n + unit - 1) // unit
+        hqn = np.zeros(n, dtype=np.uint8)
+        hqm = np.zeros((n, 16, 2), dtype=np.uint32)
+        units = np.zeros((3, nu), dtype=np.uint32)
+        raw = np.zeros((nu, unit // 2 + 1, 3), dtype=np.uint32)
+        # the taps are static in the library and every later compression writes through them: always detach
+        self.lib.gpu_model_debug_hq(hqn.ctypes.data_as(ctypes.c_void_p), hqm.ctypes.data_as(ctypes.c_void_p),
+                                    units.ctypes.data_as(ctypes.c_void_p), raw.ctypes.data_as(ctypes.c_void_p))
+        try:
+            self.compress(data, q, lgwin, **kw)
+        finally:
+            self.lib.gpu_model_debug_hq(None, None, None, None)
+        return hqn, hqm, units, raw, unit
