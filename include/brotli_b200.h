@@ -160,6 +160,9 @@ int b200_stage_match(B200Encoder* e, int quality, int lgwin, const uint8_t* in, 
 int b200_stage_hq(B200Encoder* e, int quality, int lgwin, const uint8_t* in, size_t n, uint8_t* hqn, uint32_t* hqm, uint32_t* units,
                   uint32_t* raw);
 uint32_t b200_hq_unit(B200Encoder* e, int quality, uint64_t size_hint);
+/* stage hook of the sort: the positions 0..n-1 (n <= 2^25) sorted stably by the bucket key of quality / lgwin / size n, or with
+ * level 0..2 by the key of that long-prefix level of quality 10 / 11 */
+int b200_stage_sort(B200Encoder* e, int quality, int lgwin, const uint8_t* in, size_t n, int level, uint32_t* sorted_out);
 
 #ifdef __cplusplus
 }

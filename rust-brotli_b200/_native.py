@@ -44,6 +44,8 @@ def lib():
         L.b200_stage_hq.restype = ctypes.c_int
         L.b200_hq_unit.argtypes = [vp, ctypes.c_int, ctypes.c_uint64]
         L.b200_hq_unit.restype = ctypes.c_uint32
+        L.b200_stage_sort.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp, sz, ctypes.c_int, vp]
+        L.b200_stage_sort.restype = ctypes.c_int
         _lib = L
     return _lib
 
@@ -141,3 +143,14 @@ class DeviceEncoder:
         if not ok:
             raise RuntimeError("b200_stage_hq failed")
         return hqn, hqm, units, raw, unit
+
+    def stage_sort(self, data: bytes, quality: int, lgwin: int, level=None):
+        """Positions 0..n-1 of one sort batch over `data` (n <= 2^25) in the order of the sort stage: stable by the bucket key
+        the configuration (quality, lgwin, size hint n) uses, or by the key of long-prefix level 0..2 of quality 10 / 11."""
+        import numpy as np
+        out = np.zeros(len(data), dtype=np.uint32)
+        ok = self._L.b200_stage_sort(self._h, quality, lgwin, _inptr(data), len(data), -1 if level is None else int(level),
+                                     out.ctypes.data)
+        if not ok:
+            raise RuntimeError("b200_stage_sort failed")
+        return out

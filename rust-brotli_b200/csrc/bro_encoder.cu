@@ -84,7 +84,7 @@ struct EventPool {
 // the next one (sort, match, parse) and the host<->device copies.
 struct Lane {
   cudaStream_t stream = nullptr;
-  DevBuf d_sortA, d_sortB, d_hist, d_digit, d_best, d_raw, d_unit, d_cmds, d_cmd_bits, d_lit_syms, d_cmd_syms, d_dist_syms,
+  DevBuf d_sortA, d_sortB, d_sort_state, d_best, d_raw, d_unit, d_cmds, d_cmd_bits, d_lit_syms, d_cmd_syms, d_dist_syms,
       d_hqm, d_hqn, d_hq_nodes, d_hq_pre, d_hq_scratch, d_bs_meta, d_bs_blockid, d_bs_signal, d_bs_hist, d_bs_icost, d_bs_first, d_bs_fmap, d_bs_bstart,
       d_bs_bh_in, d_bs_bh_work, d_bs_u64, d_bs_u32, d_bs_nsurv, d_cm_in, d_cm_work, d_cm_u64, d_cm_u32, d_cm_nsurv, d_cm_counts, d_cm_maps, d_dist_cost, d_mb, d_split_u8, d_split_u32, d_split_counts, d_hist_lit, d_hist_cmd, d_hist_dist, d_split_codes, d_codes_u8,
       d_codes_u16, d_hdr, d_huff_ws, d_ctxmap_ws, d_tree_ws, d_tree_bits, d_tree_nbits, d_cmd_tile, d_long_tab, d_seg_bits, d_sect_bits, d_sect_nbits;
@@ -93,7 +93,7 @@ struct Lane {
   void release() {
     DevBuf* all[] = {&d_hqm, &d_hqn, &d_hq_nodes, &d_hq_pre, &d_hq_scratch, &d_bs_meta, &d_bs_blockid, &d_bs_signal, &d_bs_hist, &d_bs_icost,
                      &d_bs_first, &d_bs_fmap, &d_bs_bstart, &d_bs_bh_in, &d_bs_bh_work, &d_bs_u64, &d_bs_u32, &d_bs_nsurv, &d_cm_in, &d_cm_work, &d_cm_u64,
-                     &d_cm_u32, &d_cm_nsurv, &d_cm_counts, &d_cm_maps, &d_dist_cost, &d_sortA, &d_sortB, &d_hist, &d_digit, &d_best, &d_raw, &d_unit, &d_cmds, &d_cmd_bits, &d_lit_syms,
+                     &d_cm_u32, &d_cm_nsurv, &d_cm_counts, &d_cm_maps, &d_dist_cost, &d_sortA, &d_sortB, &d_sort_state, &d_best, &d_raw, &d_unit, &d_cmds, &d_cmd_bits, &d_lit_syms,
                      &d_cmd_syms, &d_dist_syms, &d_mb, &d_split_u8, &d_split_u32, &d_split_counts, &d_hist_lit, &d_hist_cmd,
                      &d_hist_dist, &d_split_codes, &d_codes_u8, &d_codes_u16, &d_hdr, &d_huff_ws, &d_ctxmap_ws, &d_tree_ws,
                      &d_tree_bits, &d_tree_nbits, &d_cmd_tile, &d_long_tab, &d_seg_bits, &d_sect_bits, &d_sect_nbits};
@@ -129,10 +129,12 @@ struct B200Encoder {
   float stage_ms[B200_NUM_STAGES];
   uint32_t launches = 0;
   bool timing = false;
+  int num_sms = 0;
 
   bool init(int dev) {
     device = dev;
     CUDA_OK(cudaSetDevice(device));
+    CUDA_OK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, device));
     // (descending stream priorities per lane, to stagger the chunks, were tried: slower than equal priority)
     for (auto& L : lanes) CUDA_OK(cudaStreamCreateWithFlags(&L.stream, cudaStreamNonBlocking));
     CUDA_OK(cudaStreamCreateWithFlags(&s_in, cudaStreamNonBlocking));
@@ -221,6 +223,39 @@ struct B200Encoder {
     }
   }
 
+  // sort buffers of lane L for batches of up to nb positions: the ping-pong and the count / look-back state
+  bool ensure_sort(Lane& L, uint32_t nb) {
+    const uint32_t tiles = (nb + SORT_TILE - 1) / SORT_TILE;
+    return L.d_sortA.ensure((size_t)nb * 4 + 64) && L.d_sortB.ensure((size_t)nb * 4 + 64) &&
+           L.d_sort_state.ensure(sort_state_words(tiles) * 4);
+  }
+  // Enqueues on lane L the stable sort of the batch positions 0..count-1 (input bytes at `data`, 4096-byte aligned and padded)
+  // by the bucket key of `hash_type` (BRO_HASH_LEVEL0 + l: long-prefix level l); the sorted positions land in d_sortB.
+  // Three launches: the digit counts, then one one-sweep pass per digit.
+  template <bool LEVEL>
+  void run_sort(Lane& L, const uint8_t* data, uint32_t count, int hash_type, int key_bits) {
+    cudaStream_t stream = L.stream;
+    SortArgs sa;
+    sa.data = data;
+    sa.count = count;
+    sa.num_tiles = (count + SORT_TILE - 1) / SORT_TILE;
+    sa.state = L.d_sort_state.as<uint32_t>();
+    sa.hash_type = hash_type;
+    sa.key_bits = key_bits;
+    // counts, tile counters and look-back words start at zero for every sort (batches and chunks follow each other on the lane)
+    cudaMemsetAsync(sa.state, 0, sort_state_words(sa.num_tiles) * 4, stream);
+    sa.pass = 0;
+    sa.in = nullptr;
+    sa.outw = L.d_sortA.as<uint32_t>();
+    k_sort_count<LEVEL><<<std::min<uint32_t>(sa.num_tiles, (uint32_t)num_sms * 8), SORT_THREADS, 0, stream>>>(sa);
+    k_sort_onesweep<LEVEL><<<sa.num_tiles, SORT_THREADS, 0, stream>>>(sa);
+    sa.pass = 1;
+    sa.in = L.d_sortA.as<uint32_t>();
+    sa.outw = L.d_sortB.as<uint32_t>();
+    k_sort_onesweep<LEVEL><<<sa.num_tiles, SORT_THREADS, 0, stream>>>(sa);
+    launches += 3;
+  }
+
   // device buffers of lane L for one chunk of `c` bytes
   bool ensure_chunk(Lane& L, uint32_t c, const EncParams& P, Workspace* W) {
     const uint32_t mb_span = P.unit * P.mb_units;
@@ -280,13 +315,7 @@ struct B200Encoder {
     if (!L.d_tree_bits.ensure((size_t)NM * tree_cap * TREE_SLOT_BYTES)) return false;
     if (!L.d_tree_nbits.ensure((size_t)NM * tree_cap * 4)) return false;
     if (!L.d_sect_bits.ensure((size_t)NM * HDR_SECTIONS * SECT_BYTES) || !L.d_sect_nbits.ensure((size_t)NM * HDR_SECTIONS * 4)) return false;
-    // sort scratch
-    const uint32_t nb = std::min<uint64_t>((uint64_t)c + (1ull << P.lgwin) + 4096, kBatchMax);
-    const uint32_t tiles = (nb + SORT_TILE - 1) / SORT_TILE;
-    if (!L.d_sortA.ensure((size_t)nb * 4 + 64)) return false;
-    if (!L.d_sortB.ensure((size_t)nb * 4 + 64)) return false;
-    if (!L.d_hist.ensure((size_t)256 * tiles * 4)) return false;
-    if (!L.d_digit.ensure(512 * 4)) return false;
+    if (!ensure_sort(L, std::min<uint64_t>((uint64_t)c + (1ull << P.lgwin) + 4096, kBatchMax))) return false;
     // wire pointers
     W->lut = d_lut.as<uint32_t>();
     W->dict.words = d_dict_words.as<uint8_t>();
@@ -499,26 +528,8 @@ struct B200Encoder {
       origin &= ~4095u;  // tile staging needs word alignment
       if (origin < data_base) origin = (uint32_t)data_base;
       const uint32_t count = b1 - origin;
-      const uint32_t tiles = (count + SORT_TILE - 1) / SORT_TILE;
       mark(L, B200_ST_SORT);
-      SortArgs sa;
-      sa.data = d_all + origin;
-      sa.count = count;
-      sa.hist = L.d_hist.as<uint32_t>();
-      sa.digit_base = L.d_digit.as<uint32_t>();
-      sa.num_tiles = tiles;
-      sa.hash_type = P.hash_type;
-      sa.key_bits = P.key_bits;
-      for (int pass = 0; pass < 2; ++pass) {
-        sa.pass = pass;
-        sa.in = pass == 0 ? nullptr : L.d_sortA.as<uint32_t>();
-        sa.outw = pass == 0 ? L.d_sortA.as<uint32_t>() : L.d_sortB.as<uint32_t>();
-        k_sort_hist<false><<<tiles, SORT_THREADS, 0, stream>>>(sa);
-        k_scan_rows<<<256, 256, 0, stream>>>(sa.hist, tiles, L.d_digit.as<uint32_t>() + 256);
-        k_scan_digits<<<1, 256, 0, stream>>>(L.d_digit.as<uint32_t>() + 256, L.d_digit.as<uint32_t>());
-        k_sort_scatter<false><<<tiles, SORT_THREADS, 0, stream>>>(sa);
-        launches += 4;
-      }
+      run_sort<false>(L, d_all + origin, count, P.hash_type, P.key_bits);
       MatchArgs ma;
       ma.data = d_all;
       ma.sorted = L.d_sortB.as<uint32_t>();
@@ -554,18 +565,7 @@ struct B200Encoder {
         else if (P.depth == 1024) k_match_all<1024><<<mgrid, MATCH_THREADS, (size_t)(MATCH_THREADS + 1024) * 3 * 4, stream>>>(aa);
         else { fprintf(stderr, "[brotli_b200] unsupported bucket depth %d\n", P.depth); return false; }
         for (int lv = 0; lv < P.hq_levels; ++lv) {  // long-prefix levels: the batch re-sorted by the level's hash, lists merged
-          SortArgs sl = sa;
-          sl.hash_type = BRO_HASH_LEVEL0 + lv;
-          for (int pass = 0; pass < 2; ++pass) {
-            sl.pass = pass;
-            sl.in = pass == 0 ? nullptr : L.d_sortA.as<uint32_t>();
-            sl.outw = pass == 0 ? L.d_sortA.as<uint32_t>() : L.d_sortB.as<uint32_t>();
-            k_sort_hist<true><<<tiles, SORT_THREADS, 0, stream>>>(sl);
-            k_scan_rows<<<256, 256, 0, stream>>>(sl.hist, tiles, L.d_digit.as<uint32_t>() + 256);
-            k_scan_digits<<<1, 256, 0, stream>>>(L.d_digit.as<uint32_t>() + 256, L.d_digit.as<uint32_t>());
-            k_sort_scatter<true><<<tiles, SORT_THREADS, 0, stream>>>(sl);
-            launches += 4;
-          }
+          run_sort<true>(L, d_all + origin, count, BRO_HASH_LEVEL0 + lv, P.key_bits);
           aa.level = lv;
           aa.last_pass = lv + 1 == P.hq_levels;
           k_match_level<HQ_LEVEL_DEPTH><<<mgrid, MATCH_THREADS, (size_t)(MATCH_THREADS + HQ_LEVEL_DEPTH) * 3 * 4, stream>>>(aa);
@@ -875,6 +875,26 @@ int b200_stage_hq(B200Encoder* e, int quality, int lgwin, const uint8_t* in, siz
   ok = ok && cudaMemcpy(units, L.d_unit.p, (size_t)nu * 3 * 4, cudaMemcpyDeviceToHost) == cudaSuccess;
   ok = ok && cudaMemcpy(raw, L.d_raw.p, (size_t)nu * (P.unit / 2 + 1) * 12, cudaMemcpyDeviceToHost) == cudaSuccess;
   return ok ? 1 : 0;
+}
+
+// test hook: the sorted positions of one sort batch covering an n-byte buffer (n <= 2^25), by the bucket key the quality /
+// lgwin / size n configuration uses, or (level 0..2) by the key of that long-prefix level of quality 10 / 11
+int b200_stage_sort(B200Encoder* e, int quality, int lgwin, const uint8_t* in, size_t n, int level, uint32_t* sorted_out) {
+  if (!e || !e->ok || n == 0 || n > kBatchMax || level >= HQ_MAX_LEVELS) return 0;
+  if (cudaSetDevice(e->device) != cudaSuccess) return 0;
+  EncParams P;
+  e->fill_params(&P, quality, lgwin, n);
+  Lane& L = e->lanes[0];
+  if (!e->d_data.ensure(n + kPad) || !e->ensure_sort(L, (uint32_t)n)) return 0;
+  e->data_base = 0;
+  uint8_t* dd = e->d_data.as<uint8_t>();
+  bool ok = cudaMemcpyAsync(dd, in, n, cudaMemcpyHostToDevice, L.stream) == cudaSuccess &&
+            cudaMemsetAsync(dd + n, 0, kPad, L.stream) == cudaSuccess;
+  if (!ok) return 0;
+  if (level < 0) e->run_sort<false>(L, dd, (uint32_t)n, P.hash_type, P.key_bits);
+  else e->run_sort<true>(L, dd, (uint32_t)n, BRO_HASH_LEVEL0 + level, P.key_bits);
+  ok = cudaStreamSynchronize(L.stream) == cudaSuccess;
+  return ok && cudaMemcpy(sorted_out, L.d_sortB.p, n * 4, cudaMemcpyDeviceToHost) == cudaSuccess;
 }
 
 // parse unit the quality >= 10 path uses for this size hint with the encoder's current options (sizes the b200_stage_hq buffers)

@@ -27,6 +27,7 @@ int b200_stage_match(B200Encoder* e, int quality, int lgwin, const uint8_t* in, 
 int b200_stage_hq(B200Encoder* e, int quality, int lgwin, const uint8_t* in, size_t n, uint8_t* hqn, uint32_t* hqm, uint32_t* units,
                   uint32_t* raw);
 uint32_t b200_hq_unit(B200Encoder* e, int quality, uint64_t size_hint);
+int b200_stage_sort(B200Encoder* e, int quality, int lgwin, const uint8_t* in, size_t n, int level, uint32_t* sorted_out);
 #ifdef __cplusplus
 }
 #endif

@@ -1,8 +1,8 @@
 // bro_kernels.cuh -- CUDA kernels (sm_90a) of the brotli compression hot path.
 //
 // Stage map (DESIGN.md has the data layout and the per-kernel roofline):
-//   sort    k_sort_hist / k_scan_rows / k_scan_digits / k_sort_scatter   stable LSD radix sort of positions by
-//                                                                        bucket key  (replaces hasher Store*)
+//   sort    k_sort_count / k_sort_onesweep (x2)   stable one-sweep LSD radix sort of positions by bucket key
+//                                                 (replaces hasher Store*)
 //   match   k_match          every position vs the `depth` most recent earlier positions of its bucket
 //                            (replaces the bucket walk of FindLongestMatch, backward_references/mod.rs:1754-1792)
 //   parse   k_parse          greedy+lazy parse per unit (CreateBackwardReferences mod.rs:2376)
@@ -190,21 +190,35 @@ __device__ __forceinline__ void tma_stage_tile(void* smem_dst, const void* gmem_
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Radix sort of the positions of one batch by bucket key (stable => ascending position inside a bucket).
-// Pass 0 sorts by key & 0xFF reading the input bytes; pass 1 by key >> 8 reading the packed words of pass 0.
-// Element word: (key >> 8) << 25 | (position - batch_origin).
+// Radix sort of the positions of one batch by bucket key (stable => ascending position inside a bucket): a one-sweep LSD sort
+// with two digits, key & 0xFF and then key >> 8 (7 bits for 15-bit keys, 6 for 14-bit ones).
+//   k_sort_count     reads the input bytes once (TMA-staged tiles) and counts both digits over the whole batch; its last CTA turns
+//                    the counts into each digit's base offset
+//   k_sort_onesweep  one pass: ranks a tile's elements in shared memory, finds the tile's offset of every digit by a decoupled
+//                    look-back over the tiles before it, and writes the tile out in digit order (runs of consecutive addresses)
+// Pass 0 takes its keys from the staged input and writes the element word (key >> 8) << 25 | (position - batch_origin);
+// pass 1 reads those words and writes plain batch-relative positions.
 // ---------------------------------------------------------------------------------------------------
 #define SORT_THREADS 256
 #define SORT_ITEMS 16
 #define SORT_TILE (SORT_THREADS * SORT_ITEMS)
+// sort state of a lane (32-bit words), zeroed before every sort
+#define SORT_ST_COUNT 0     // [2][256] digit counts of pass 0 / pass 1 over the batch
+#define SORT_ST_BASE 512    // [2][256] first output index of each digit
+#define SORT_ST_DONE 1024   // k_sort_count CTAs that have added their counts
+#define SORT_ST_TILE 1025   // [2] next tile index of each pass
+#define SORT_ST_FLAGS 1056  // [2][num_tiles][256] look-back words: flag bits | count
+#define SORT_LB_AGG (1u << 30)  // count of the digit in this tile alone
+#define SORT_LB_INC (2u << 30)  // count of the digit in this tile and every tile before it
+#define SORT_LB_VAL 0x3FFFFFFFu
+__host__ __device__ constexpr size_t sort_state_words(uint32_t num_tiles) { return SORT_ST_FLAGS + (size_t)2 * num_tiles * 256; }
 
 struct SortArgs {
   const uint8_t* data;   // data + batch_origin
   uint32_t count;        // positions in batch (halo + payload)
   const uint32_t* in;    // pass 1 input
   uint32_t* outw;        // pass output
-  uint32_t* hist;        // [256][num_tiles]
-  const uint32_t* digit_base;  // [256]
+  uint32_t* state;       // [sort_state_words(num_tiles)], zeroed
   uint32_t num_tiles;
   int hash_type, key_bits;
   int pass;
@@ -229,91 +243,118 @@ __device__ __forceinline__ uint32_t smem_key(const uint32_t* sw, uint32_t e, int
   return hash_key_from_words(hash_type, key_bits, lo, hi);
 }
 
-__device__ __forceinline__ void sort_stage_tile(const SortArgs& a, uint32_t tile, uint32_t* sw, uint64_t* bar) {
-  // stage SORT_TILE + 48 bytes with one TMA bulk copy (the input is padded, so reading past `count` is safe; the batch origin
-  // is 4096-byte aligned)
-  tma_stage_tile(sw, a.data + (size_t)tile * SORT_TILE, SORT_TILE + 48, bar);
-}
-
-template <bool LEVEL>
-__global__ void __launch_bounds__(SORT_THREADS) k_sort_hist(SortArgs a) {
-  __shared__ __align__(16) uint32_t sw[SORT_TILE / 4 + 12];
-  __shared__ __align__(8) uint64_t s_bar;
-  __shared__ uint32_t sh[256];
-  const uint32_t tile = blockIdx.x;
-  sh[threadIdx.x] = 0;
-  if (a.pass == 0) sort_stage_tile(a, tile, sw, &s_bar);
-  __syncthreads();
-  const uint32_t base = tile * SORT_TILE;
-#pragma unroll 4
-  for (int r = 0; r < SORT_ITEMS; ++r) {
-    uint32_t e = r * SORT_THREADS + threadIdx.x;
-    if (base + e < a.count) {
-      uint32_t digit;
-      if (a.pass == 0) digit = smem_key<LEVEL>(sw, e, a.hash_type, a.key_bits) & 0xFFu;
-      else digit = a.in[base + e] >> 25;
-      atomicAdd(&sh[digit], 1u);
-    }
-  }
-  __syncthreads();
-  a.hist[(size_t)threadIdx.x * a.num_tiles + tile] = sh[threadIdx.x];
-}
-
-// exclusive scan of each digit row over tiles; row totals to totals[digit]
-__global__ void __launch_bounds__(256) k_scan_rows(uint32_t* hist, uint32_t num_tiles, uint32_t* totals) {
-  __shared__ uint32_t s_warp[8];
-  __shared__ uint32_t s_carry;
-  uint32_t* row = hist + (size_t)blockIdx.x * num_tiles;
-  if (threadIdx.x == 0) s_carry = 0;
-  __syncthreads();
-  for (uint32_t base = 0; base < num_tiles; base += 256) {
-    uint32_t i = base + threadIdx.x;
-    uint32_t v = i < num_tiles ? row[i] : 0;
-    uint32_t x = v;
-    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-      if (lane >= (uint32_t)o) x += y;
-    }
-    if (lane == 31) s_warp[wid] = x;
-    __syncthreads();
-    uint32_t woff = 0;
-    for (uint32_t w = 0; w < wid; ++w) woff += s_warp[w];
-    uint32_t carry = s_carry;
-    if (i < num_tiles) row[i] = carry + woff + x - v;
-    __syncthreads();
-    if (threadIdx.x == 255) s_carry = carry + woff + x;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) totals[blockIdx.x] = s_carry;
-}
-__global__ void __launch_bounds__(256) k_scan_digits(const uint32_t* totals, uint32_t* digit_base) {
-  __shared__ uint32_t s[256];
-  s[threadIdx.x] = totals[threadIdx.x];
-  __syncthreads();
+// TMA bulk copy of tile `tile` (SORT_TILE + 48 bytes: the input is padded, so reading past `count` is safe; the batch origin is
+// 4096-byte aligned) into sw; the whole CTA calls this and waits on phase `parity` of the (already initialised) barrier
+__device__ __forceinline__ void sort_stage_tile(const SortArgs& a, uint32_t tile, uint32_t* sw, uint64_t* bar, uint32_t parity) {
   if (threadIdx.x == 0) {
-    uint32_t acc = 0;
-    for (int i = 0; i < 256; ++i) { uint32_t v = s[i]; s[i] = acc; acc += v; }
+    mbar_expect_tx(bar, SORT_TILE + 48);
+    tma_load_1d(sw, a.data + (size_t)tile * SORT_TILE, SORT_TILE + 48, bar);
   }
-  __syncthreads();
-  digit_base[threadIdx.x] = s[threadIdx.x];
+  mbar_wait(bar, parity);
 }
 
+// exclusive prefix sum over the CTA's 256 threads (s_warp: 8 words of shared memory); all threads call it
+__device__ __forceinline__ uint32_t block_excl_scan256(uint32_t v, uint32_t* s_warp) {
+  const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  uint32_t x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= (uint32_t)o) x += y;
+  }
+  if (lane == 31) s_warp[wid] = x;
+  __syncthreads();
+  uint32_t woff = 0;
+  for (uint32_t w = 0; w < wid; ++w) woff += s_warp[w];
+  return woff + x - v;
+}
+
+// Look-back words carry their own count, so nothing is read after them that their publication has to order; relaxed loads let
+// SORT_LB_WINDOW of them be in flight at once (both passes of a 29 M-position batch on an H100 80GB HBM3 at 700 W: 587 µs, against
+// 622 µs with one acquire load per step).
+#define SORT_LB_WINDOW 8
+__device__ __forceinline__ uint32_t ld_relaxed_gpu(const uint32_t* p) {
+  uint32_t v;
+  asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_release_gpu(uint32_t* p, uint32_t v) {
+  asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+
+// grid-stride over the tiles; a.state zeroed
 template <bool LEVEL>
-__global__ void __launch_bounds__(SORT_THREADS, 6) k_sort_scatter(SortArgs a) {
+__global__ void __launch_bounds__(SORT_THREADS) k_sort_count(SortArgs a) {
   __shared__ __align__(16) uint32_t sw[SORT_TILE / 4 + 12];
   __shared__ __align__(8) uint64_t s_bar;
-  __shared__ uint32_t wc[SORT_THREADS / 32][256];
-  __shared__ uint32_t s_word[SORT_TILE];  // element words parked in shared memory (keeps the register count low => occupancy)
-  const uint32_t tile = blockIdx.x;
-  const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  for (uint32_t i = threadIdx.x; i < (SORT_THREADS / 32) * 256; i += SORT_THREADS) (&wc[0][0])[i] = 0;
-  if (a.pass == 0) sort_stage_tile(a, tile, sw, &s_bar);
+  __shared__ uint32_t sh[2][256];
+  __shared__ uint32_t s_warp[SORT_THREADS / 32];
+  __shared__ bool s_last;
+  const uint32_t tid = threadIdx.x;
+  sh[0][tid] = 0;
+  sh[1][tid] = 0;
+  if (tid == 0) mbar_init(&s_bar, 1);
   __syncthreads();
+  uint32_t parity = 0;
+  for (uint32_t tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x, parity ^= 1u) {
+    sort_stage_tile(a, tile, sw, &s_bar, parity);
+    const uint32_t base = tile * SORT_TILE;
+#pragma unroll 4
+    for (int r = 0; r < SORT_ITEMS; ++r) {
+      const uint32_t e = r * SORT_THREADS + tid;
+      if (base + e < a.count) {
+        const uint32_t key = smem_key<LEVEL>(sw, e, a.hash_type, a.key_bits);
+        atomicAdd(&sh[0][key & 0xFFu], 1u);
+        atomicAdd(&sh[1][key >> 8], 1u);
+      }
+    }
+    __syncthreads();  // sw is read before the next tile's copy lands in it
+  }
+  if (sh[0][tid]) atomicAdd(&a.state[SORT_ST_COUNT + tid], sh[0][tid]);
+  if (sh[1][tid]) atomicAdd(&a.state[SORT_ST_COUNT + 256 + tid], sh[1][tid]);
+  __threadfence();
+  __syncthreads();
+  if (tid == 0) s_last = atomicAdd(&a.state[SORT_ST_DONE], 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();  // every other CTA's counts are in
+  for (int p = 0; p < 2; ++p) {
+    const uint32_t c = __ldcg(&a.state[SORT_ST_COUNT + p * 256 + tid]);
+    a.state[SORT_ST_BASE + p * 256 + tid] = block_excl_scan256(c, s_warp);
+    __syncthreads();  // s_warp is reused
+  }
+}
+
+// one pass; one tile per CTA, taken in order from the state's tile counter
+template <bool LEVEL>
+__global__ void __launch_bounds__(SORT_THREADS, 4) k_sort_onesweep(SortArgs a) {
+  __shared__ __align__(16) uint32_t s_buf[SORT_TILE];  // pass 0: the staged input bytes; then the tile's words in digit order
+  __shared__ uint8_t s_dig[SORT_TILE];                  // digit of each word of s_buf
+  __shared__ uint32_t wc[SORT_THREADS / 32][256];       // per warp and digit: count, then the first slot of s_buf
+  __shared__ uint32_t s_gofs[256];                      // per digit: output index minus slot
+  __shared__ uint32_t s_warp[SORT_THREADS / 32];
+  __shared__ uint32_t s_tile;
+  __shared__ __align__(8) uint64_t s_bar;
+  const uint32_t tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int nbits = a.pass == 0 ? 8 : a.key_bits - 8;
+  for (uint32_t i = tid; i < (SORT_THREADS / 32) * 256; i += SORT_THREADS) (&wc[0][0])[i] = 0;
+  if (tid == 0) {
+    s_tile = atomicAdd(&a.state[SORT_ST_TILE + a.pass], 1u);
+    if (a.pass == 0) mbar_init(&s_bar, 1);
+  }
+  __syncthreads();
+  const uint32_t tile = s_tile;
+  if (a.pass == 0) sort_stage_tile(a, tile, s_buf, &s_bar, 0);
   const uint32_t base = tile * SORT_TILE;
-  uint16_t lrank[SORT_ITEMS];
-  uint8_t dig[SORT_ITEMS];
+  uint32_t word[SORT_ITEMS];
+  uint32_t rk[SORT_ITEMS];  // digit << 16 | rank among the warp's elements of that digit; ~0u past the end of the batch
+  if (a.pass == 1) {  // all loads in flight before the ranking (its __syncwarp()s would keep them one round apart)
+#pragma unroll
+    for (int r = 0; r < SORT_ITEMS; ++r) {
+      const uint32_t e = wid * (32 * SORT_ITEMS) + r * 32 + lane;
+      word[r] = base + e < a.count ? a.in[base + e] : 0u;
+    }
+  }
   // element order inside the tile: warp-major, then round, then lane  (=> ascending position)
 #pragma unroll
   for (int r = 0; r < SORT_ITEMS; ++r) {
@@ -322,54 +363,93 @@ __global__ void __launch_bounds__(SORT_THREADS, 6) k_sort_scatter(SortArgs a) {
     uint32_t digit = 0x100u, w = 0;
     if (valid) {
       if (a.pass == 0) {
-        const uint32_t key = smem_key<LEVEL>(sw, e, a.hash_type, a.key_bits);
+        const uint32_t key = smem_key<LEVEL>(s_buf, e, a.hash_type, a.key_bits);
         digit = key & 0xFFu;
         w = ((key >> 8) << 25) | (base + e);
       } else {
-        const uint32_t v = a.in[base + e];
+        const uint32_t v = word[r];
         digit = v >> 25;
         w = v & 0x1FFFFFFu;
       }
     }
-    s_word[e] = w;
-#ifdef SORT_USE_MATCH_ANY
-    const uint32_t peers = __match_any_sync(0xffffffffu, digit);
-#else
-    // lanes with the same digit, from 9 ballots (MATCH.ANY measured slower: it goes through the MIO queue)
+    // lanes with the same digit, from 1 + nbits ballots (MATCH.ANY measured slower: it goes through the MIO queue)
     uint32_t peers = __ballot_sync(0xffffffffu, valid);
     if (!valid) peers = ~peers;
 #pragma unroll
     for (int b = 0; b < 8; ++b) {
-      const bool bit = (digit >> b) & 1u;
-      const uint32_t bal = __ballot_sync(0xffffffffu, bit);
-      peers &= bit ? bal : ~bal;
+      if (b < nbits) {
+        const bool bit = (digit >> b) & 1u;
+        const uint32_t bal = __ballot_sync(0xffffffffu, bit);
+        peers &= bit ? bal : ~bal;
+      }
     }
-#endif
     const uint32_t rank_in_round = __popc(peers & ((1u << lane) - 1u));
     uint32_t old = 0;
     if (valid) old = wc[wid][digit];
     __syncwarp();
     if (valid && rank_in_round == 0) wc[wid][digit] = old + __popc(peers);
     __syncwarp();
-    dig[r] = (uint8_t)digit;
-    lrank[r] = valid ? (uint16_t)(old + rank_in_round) : (uint16_t)0xFFFF;
+    word[r] = w;
+    rk[r] = valid ? (digit << 16) | (old + rank_in_round) : ~0u;
   }
   __syncthreads();
-  {  // per digit: exclusive scan over warps, seeded with the global offset of (digit, tile)
-    const uint32_t d = threadIdx.x;
-    uint32_t acc = a.digit_base[d] + a.hist[(size_t)d * a.num_tiles + tile];
+  // per digit d: the tile's count, its first slot in the tile, and the first slot of each warp's elements
+  const uint32_t d = tid;
+  uint32_t agg = 0;
+#pragma unroll
+  for (int w = 0; w < SORT_THREADS / 32; ++w) agg += wc[w][d];
+  const uint32_t first = block_excl_scan256(agg, s_warp);
+  {
+    uint32_t acc = first;
+#pragma unroll
     for (int w = 0; w < SORT_THREADS / 32; ++w) {
       const uint32_t t = wc[w][d];
       wc[w][d] = acc;
       acc += t;
     }
   }
-  __syncthreads();
+  if (d < (1u << nbits)) {  // decoupled look-back: this digit's count in the tiles before this one
+    uint32_t* flags = a.state + SORT_ST_FLAGS + (size_t)a.pass * a.num_tiles * 256;
+    uint32_t before = 0;
+    if (tile == 0) {
+      st_release_gpu(flags + d, SORT_LB_INC | agg);
+    } else {
+      st_release_gpu(flags + (size_t)tile * 256 + d, SORT_LB_AGG | agg);
+      // Tiles are handed out in order by an atomic counter, so every tile before this one was claimed by a CTA that is already
+      // running, and that CTA publishes its aggregate before it waits on anything.  Tile 0 publishes its inclusive count
+      // without waiting.  So each word this loop waits on gets written, and the walk ends at tile 0 at the latest.
+      uint32_t t = tile;  // tiles t - 1, t - 2, ... are still to be added
+      bool done = false;
+      while (!done) {
+        uint32_t v[SORT_LB_WINDOW];
+#pragma unroll
+        for (uint32_t j = 0; j < SORT_LB_WINDOW; ++j) v[j] = j < t ? ld_relaxed_gpu(flags + (size_t)(t - 1 - j) * 256 + d) : 0u;
+        uint32_t j = 0;
+#pragma unroll
+        for (; j < SORT_LB_WINDOW; ++j) {
+          if (v[j] == 0) break;  // not published yet: read again from here
+          before += v[j] & SORT_LB_VAL;
+          if (v[j] & SORT_LB_INC) { done = true; break; }
+        }
+        t -= j;
+      }
+      st_release_gpu(flags + (size_t)tile * 256 + d, SORT_LB_INC | (before + agg));
+    }
+    s_gofs[d] = a.state[SORT_ST_BASE + a.pass * 256 + d] + before - first;
+  }
+  __syncthreads();  // (pass 0: every key is computed before s_buf is overwritten)
 #pragma unroll
   for (int r = 0; r < SORT_ITEMS; ++r) {
-    const uint32_t e = wid * (32 * SORT_ITEMS) + r * 32 + lane;
-    if (lrank[r] != 0xFFFF) a.outw[wc[wid][dig[r]] + lrank[r]] = s_word[e];
+    if (rk[r] != ~0u) {
+      const uint32_t dg = rk[r] >> 16;
+      const uint32_t slot = wc[wid][dg] + (rk[r] & 0xFFFFu);
+      s_buf[slot] = word[r];
+      s_dig[slot] = (uint8_t)dg;
+    }
   }
+  __syncthreads();
+  const uint32_t n_tile = min((uint32_t)SORT_TILE, a.count - base);
+  for (uint32_t i = tid; i < n_tile; i += SORT_THREADS) a.outw[s_gofs[s_dig[i]] + i] = s_buf[i];
 }
 
 // unaligned little-endian loads built from aligned words (the input has >= 512 readable bytes of padding)
