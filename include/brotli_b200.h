@@ -153,8 +153,11 @@ int b200_encoder_compress_range(B200Encoder* e, int quality, int lgwin, uint64_t
                                 size_t range_start, size_t range_len, int first, int last, int byte_align, uint8_t* out,
                                 size_t out_cap, size_t* out_size, int device_io);
 int b200_encoder_last_timings(B200Encoder* e, float* ms, uint32_t* launches);
-/* stage hook used by the parity tests: per-position best bucket match (distance << 8 | capped length) */
-int b200_stage_match(B200Encoder* e, int quality, int lgwin, const uint8_t* in, size_t n, uint32_t* best_out);
+/* stage hook of quality 5..9: best[] of the match stage (distance << 8 | capped length, or a static-dictionary candidate) for
+ * [range_start, range_start + range_len) of an n-byte buffer, range_len <= one chunk; size_hint 0 = n.  search = 0: the up-front
+ * kernels; search = 1: the on-demand search at every position (returns 0 where that path does not run: depth < 64, two batches) */
+int b200_stage_match(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n, size_t range_start,
+                     size_t range_len, int search, uint32_t* best_out);
 /* stage hook of quality 10 / 11 (n <= one chunk): matches per position hqn[n], hqm[n][16][2] (distance, length word); per parse
  * unit ncmd, tail, ncopy as units[3][nu]; raw commands raw[nu][unit / 2 + 1][3].  b200_hq_unit gives the unit for size_hint n. */
 int b200_stage_hq(B200Encoder* e, int quality, int lgwin, const uint8_t* in, size_t n, uint8_t* hqn, uint32_t* hqm, uint32_t* units,

@@ -38,7 +38,7 @@ def lib():
                                                   ctypes.c_int, ctypes.c_int, vp, sz, ctypes.POINTER(sz), ctypes.c_int]
         L.b200_encoder_compress_range.restype = ctypes.c_int
         L.b200_encoder_last_timings.argtypes = [vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_uint32)]
-        L.b200_stage_match.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp, sz, vp]
+        L.b200_stage_match.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.c_uint64, vp, sz, sz, sz, ctypes.c_int, vp]
         L.b200_stage_match.restype = ctypes.c_int
         L.b200_stage_hq.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp, sz, vp, vp, vp, vp]
         L.b200_stage_hq.restype = ctypes.c_int
@@ -117,10 +117,17 @@ class DeviceEncoder:
         self._L.b200_encoder_last_timings(self._h, ms, ctypes.byref(launches))
         return dict(zip(STAGE_NAMES, [float(x) for x in ms])), int(launches.value)
 
-    def stage_match(self, data: bytes, quality: int, lgwin: int):
+    def stage_match(self, data: bytes, quality: int, lgwin: int, size_hint: int = 0, start: int = 0, length=None,
+                    on_demand: bool = False):
+        """best[] of the quality 5..9 match stage for data[start:start + length] (length <= 24 MiB; the bytes in front of start
+        are its window), as the up-front kernels compute it, or (on_demand) as the on-demand search computes it at every
+        position -- which needs bucket depth >= 64 and a range that fits one sort batch.  size_hint 0 = len(data)."""
         import numpy as np
-        out = np.zeros(len(data), dtype=np.uint32)
-        ok = self._L.b200_stage_match(self._h, quality, lgwin, _inptr(data), len(data), out.ctypes.data)
+        if length is None:
+            length = len(data) - start
+        out = np.zeros(length, dtype=np.uint32)
+        ok = self._L.b200_stage_match(self._h, quality, lgwin, size_hint, _inptr(data), len(data), start, length, int(on_demand),
+                                      out.ctypes.data)
         if not ok:
             raise RuntimeError("b200_stage_match failed")
         return out

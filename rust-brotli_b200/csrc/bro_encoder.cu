@@ -122,6 +122,8 @@ struct B200Encoder {
   cudaStream_t s_in = nullptr, s_out = nullptr;  // copy streams
   DevBuf d_dict_words, d_dict_hash, d_dict_lutb, d_dict_lute, d_dict_trg, d_dict_tr;
   DevBuf d_data, d_lut, d_out, d_total;          // d_total: [0] running bit position, [1 + k] position after chunk k
+  DevBuf d_probe;                                // b200_stage_match(search = 1): the on-demand search at every position
+  uint32_t* od_probe = nullptr;                  // set only inside that hook: run_chunk launches k_od_probe into it
   uint64_t* h_total = nullptr;                   // pinned mirror of d_total[1 + k]
   size_t h_total_cap = 0;
   EventPool sync_events;
@@ -165,7 +167,7 @@ struct B200Encoder {
     cudaSetDevice(device);
     cudaDeviceSynchronize();
     for (auto& L : lanes) L.release();
-    DevBuf* all[] = {&d_data, &d_lut, &d_out, &d_total, &d_dict_words, &d_dict_hash, &d_dict_lutb, &d_dict_lute, &d_dict_trg, &d_dict_tr};
+    DevBuf* all[] = {&d_data, &d_lut, &d_out, &d_total, &d_probe, &d_dict_words, &d_dict_hash, &d_dict_lutb, &d_dict_lute, &d_dict_trg, &d_dict_tr};
     for (auto* b : all) b->release();
     if (h_total) cudaFreeHost(h_total);
     sync_events.destroy();
@@ -552,6 +554,12 @@ struct B200Encoder {
         da.m = ma;
         da.sig = L.d_sortA.as<uint32_t>();
         k_rank_sig<<<(count + 255) / 256, 256, 0, stream>>>(ma, L.d_sortA.as<uint32_t>());
+        if (od_probe) {  // stage hook only: the search of every position, while the ranks and signatures are intact
+          const uint32_t pg = (range_len + 7) / 8;
+          if (P.depth == 64) k_od_probe<64><<<pg, 256, 0, stream>>>(da, range_start, range_len, od_probe);
+          else if (P.depth == 128) k_od_probe<128><<<pg, 256, 0, stream>>>(da, range_start, range_len, od_probe);
+          else k_od_probe<256><<<pg, 256, 0, stream>>>(da, range_start, range_len, od_probe);
+        }
       } else
       if (P.quality >= 10) {  // all matches of every position
         MatchAllArgs aa;
@@ -844,16 +852,38 @@ int b200_encoder_last_timings(B200Encoder* e, float* ms, uint32_t* launches) {
   return 1;
 }
 
-// test hook: device results of the match stage for an n-byte buffer (host in, host out); n <= one chunk
-int b200_stage_match(B200Encoder* e, int quality, int lgwin, const uint8_t* in, size_t n, uint32_t* best_out) {
-  if (!e || !e->ok || n == 0 || n > kChunk) return 0;
+// test hook (quality 5..9): best[] of the match stage for the range [range_start, range_start + range_len) of an n-byte buffer
+// (host in, host out; range_len <= one chunk, the bytes in front of the range are its window).  search = 0: the up-front kernels
+// (k_match_shallow / k_match_deep), with the on-demand path switched off for the call.  search = 1: the on-demand search
+// (k_rank_sig + deep_best_warp) at every position of the range; 0 is returned where that path does not run (depth < 64, or a
+// chunk that needs more than one sort batch).
+int b200_stage_match(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n, size_t range_start,
+                     size_t range_len, int search, uint32_t* best_out) {
+  if (!e || !e->ok || n == 0 || n >= 0xFFFFF000ull || range_len == 0 || range_len > kChunk || range_start > n - range_len) return 0;
+  if (b200_effective_quality(quality) >= 10 || (search != 0 && search != 1)) return 0;
   if (cudaSetDevice(e->device) != cudaSuccess) return 0;
+  if (!size_hint) size_hint = n;
+  if (search) {
+    EncParams P;
+    e->fill_params(&P, quality, lgwin, size_hint);
+    const uint64_t payload_max = kBatchMax - (1ull << P.lgwin) - 4096;
+    if (P.depth < 64 || range_len > payload_max) return 0;
+    if (!e->d_probe.ensure(range_len * 4)) return 0;
+    e->od_probe = e->d_probe.as<uint32_t>();
+  }
+  const int ondemand = e->ondemand;
+  e->ondemand = search ? 2 : 0;
   size_t got = 0;
-  if (!compress_range_impl(e, quality, lgwin, n, in, n, 0, n, true, true, false, nullptr, b200_max_compressed_size(n) + 64, &got, 0, true)) {
+  const bool ok = compress_range_impl(e, quality, lgwin, size_hint, in, n, range_start, range_len, true, true, false, nullptr,
+                                      b200_max_compressed_size(range_len) + 64, &got, 0, true);
+  e->ondemand = ondemand;
+  e->od_probe = nullptr;
+  if (!ok) {
     cudaDeviceSynchronize();
     return 0;
   }
-  return cudaMemcpy(best_out, e->lanes[0].d_best.p, n * 4, cudaMemcpyDeviceToHost) == cudaSuccess;
+  const void* src = search ? e->d_probe.p : e->lanes[0].d_best.p;
+  return cudaMemcpy(best_out, src, range_len * 4, cudaMemcpyDeviceToHost) == cudaSuccess;
 }
 
 // test hook (quality >= 10): matches per position, per-unit results and raw commands of an n-byte buffer (n <= one chunk)

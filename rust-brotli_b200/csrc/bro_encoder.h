@@ -23,7 +23,8 @@ int b200_encoder_compress_range(B200Encoder* e, int quality, int lgwin, uint64_t
                                 size_t range_start, size_t range_len, int first, int last, int byte_align, uint8_t* out,
                                 size_t out_cap, size_t* out_size, int device_io);
 int b200_encoder_last_timings(B200Encoder* e, float* ms /* [B200_NUM_STAGES] */, uint32_t* launches);
-int b200_stage_match(B200Encoder* e, int quality, int lgwin, const uint8_t* in, size_t n, uint32_t* best_out);
+int b200_stage_match(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n, size_t range_start,
+                     size_t range_len, int search, uint32_t* best_out);
 int b200_stage_hq(B200Encoder* e, int quality, int lgwin, const uint8_t* in, size_t n, uint8_t* hqn, uint32_t* hqm, uint32_t* units,
                   uint32_t* raw);
 uint32_t b200_hq_unit(B200Encoder* e, int quality, uint64_t size_hint);

@@ -1464,6 +1464,21 @@ __device__ __forceinline__ uint32_t deep_best_warp(const DeepArgs& A, uint32_t p
   return res;
 }
 
+// Test probe of the on-demand search: deep_best_warp() at every position of [start, start + len), one warp per position, into
+// out[len].  Launched right after k_rank_sig (while the ranks, signatures and sorted list are intact) only when a stage hook asks.
+template <int DEPTH>
+__global__ void __launch_bounds__(256) k_od_probe(DeepArgs A, uint32_t start, uint32_t len, uint32_t* out) {
+  __shared__ uint32_t s_back_all[8][256];
+  const uint32_t w = blockIdx.x * 8u + (threadIdx.x >> 5);
+  if (w >= len) return;
+  const uint32_t p = start + w;
+  const uint32_t r = A.m.best[p];
+  uint32_t cpos[DEPTH / 32], csig[DEPTH / 32];
+  deep_fetch<DEPTH>(A, r, cpos, csig);
+  const uint32_t b = deep_best_warp<DEPTH>(A, p, r, cpos, csig, s_back_all[threadIdx.x >> 5]);
+  if ((threadIdx.x & 31) == 0) out[w] = b;
+}
+
 // find_match() of bro_parse.cuh at the range-relative position pos, whole warp: lane i probes cached distance i, then the bucket
 template <int NL, int DEPTH>
 __device__ __forceinline__ bool find_match_ondemand(const EncParams& P, const DeepArgs& A, const uint8_t* data, const int32_t* dca,

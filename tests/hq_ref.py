@@ -33,11 +33,11 @@ def _words(a, pad):
     return w64 & np.uint64(0xFFFFFFFF), w64
 
 
-def _lcp(w64, p, c, cap):
-    """Common-prefix length of positions p and c (arrays), at most cap."""
+def _lcp(w64, p, c, cap, limit=LCAP):
+    """Common-prefix length of positions p and c (arrays), at most cap (<= limit, the largest cap of the caller)."""
     out = np.zeros(len(p), dtype=np.int64)
     alive = np.arange(len(p))
-    for j in range(0, LCAP, 8):
+    for j in range(0, limit, 8):
         if not alive.size:
             break
         x = w64[p[alive] + j] ^ w64[c[alive] + j]
@@ -60,10 +60,11 @@ def _level_hash(w64, nbytes):
     return h
 
 
-def _nearest_same_key(key, query, depth, accept, w64, maxl):
+def _nearest_same_key(key, query, depth, accept, w64, maxl, limit=LCAP, maxb=None):
     """(p, distance, length) for every query position p and each of the `depth` nearest earlier positions with the same key
     for which accept(p, cand) holds.  A position stops collecting once it has a match of length maxl: nothing farther can
-    be longer, so the fronts do not change."""
+    be longer, so the fronts do not change.  With maxb (per position) it also stops at the first entry farther back than
+    maxb[p]: every older one is out of the window too."""
     order = np.argsort(key, kind="stable")
     rank = np.empty(len(key), dtype=np.int64)
     rank[order] = np.arange(len(key))
@@ -77,10 +78,13 @@ def _nearest_same_key(key, query, depth, accept, w64, maxl):
         c = order[r - k]
         same = key[c] == key[q]
         q, r, c = q[same], r[same], c[same]  # the rest have fewer than k earlier entries in their bucket
+        if maxb is not None:
+            inw = q - c <= maxb[q]
+            q, r, c = q[inw], r[inw], c[inw]
         if not q.size:
             break
         a = accept(q, c)
-        ln = _lcp(w64, q[a], c[a], maxl[q[a]])
+        ln = _lcp(w64, q[a], c[a], maxl[q[a]], limit)
         ps.append(q[a]); ds.append(q[a] - c[a]); ls.append(ln)
         full = np.zeros(len(q), dtype=bool)
         full[np.flatnonzero(a)[ln == maxl[q[a]]]] = True

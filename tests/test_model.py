@@ -213,3 +213,48 @@ def test_model_hq_edge_sizes(model, q, n):
     d = (golden_bytes("alice29.txt") * 2)[:n]
     c, _ = model.compress(d, q, 22)
     assert sys_decompress(c, max(n, 1)) == d
+
+
+def _model_best(model, d, q, w, hint=0, start=0, length=None):
+    import numpy as np
+    length = len(d) - start if length is None else length
+    best = np.zeros(length + 1, dtype=np.uint32)
+    model.compress_range(d, start, length, q, w, True, True, False, size_hint=hint, best_out=best.ctypes.data)
+    return best[:length]
+
+
+def test_model_match_stage_equals_brute_force(model):
+    """best[] of quality 5..9 (the model's sequential bucket rings) against tests/match_ref.py, a numpy restatement of the
+    stage's contract that shares no code with the kernels' headers: every hasher / key width / depth of ChooseHasher, planted
+    edges at lgwin 10, 12, 16 and 22, English text (dictionary words) and ranges whose window lies in front of them."""
+    import numpy as np
+    import match_ref
+    alice = golden_bytes("alice29.txt")[:40000]
+    mib = 1 << 20
+    cases = [(alice, q, w, h) for q, w, h in ((5, 22, mib), (5, 22, 2 * mib), (5, 22, 8 * mib), (6, 22, mib), (6, 22, 8 * mib),
+                                              (7, 22, 2 * mib), (7, 22, 8 * mib), (8, 22, mib), (9, 22, mib), (5, 16, 0), (8, 16, 0),
+                                              (6, 10, 0), (6, 12, 0))]
+    cases += [(match_ref.planted_input(10), 6, 10, 0), (match_ref.planted_input(12), 6, 12, 0), (match_ref.planted_input(16), 5, 16, 0),
+              (match_ref.planted_input(16), 9, 16, 0)]
+    seen = set()
+    for d, q, w, h in cases:
+        ref = match_ref.match_ref(d, q, w, h)
+        diff = match_ref.first_difference(ref, _model_best(model, d, q, w, h))
+        assert diff is None, "q%d lgwin %d hint %d n=%d: %s" % (q, w, h, len(d), diff)
+        seen.add(match_ref.config(q, w, h or len(d)))
+        assert (ref & 0x80).any() and ((ref != 0) & (ref & 0x80 == 0)).sum() > 1000  # dictionary and bucket matches
+    assert len(seen) == 10  # H5/14/16, H5/15/16, H6/15/16, H5/14/32, H6/15/32, H5/15/64, H6/15/64, H5/15/128, H9/15/256, H6/15/256
+    # lgwin 22 (H6, 16 deep: the size is above 4 MiB): the planted positions, the window edge and a sample
+    d, marks = match_ref.planted_input(22, with_positions=True)
+    maxb = (1 << 22) - 16
+    rng = np.random.default_rng(1)
+    query = np.unique(np.concatenate([marks, np.arange(maxb, maxb + 4096), rng.integers(0, len(d), 50000), np.arange(len(d) - 64, len(d))]))
+    ref = match_ref.match_ref(d, 5, 22, query=query)
+    diff = match_ref.first_difference(ref, _model_best(model, d, 5, 22)[query], query)
+    assert diff is None, "planted lgwin 22: %s" % diff
+    # ranges with a window in front of them
+    pl = match_ref.planted_input(16) + golden_bytes("alice29.txt")
+    for q, w, start, length in ((5, 18, 4113, 70001), (9, 16, 65536 + 12345, 30001)):
+        ref = match_ref.match_ref(pl, q, w, 0, start, length)
+        diff = match_ref.first_difference(ref, _model_best(model, pl, q, w, 0, start, length), np.arange(start, start + length))
+        assert diff is None, "q%d lgwin %d range %d+%d: %s" % (q, w, start, length, diff)

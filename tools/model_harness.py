@@ -37,7 +37,7 @@ class Model:
         self.lib.gpu_model_default_params(ctypes.byref(p), q, lgwin, n, size_hint)
         for k, v in kw.items(): setattr(p, k, v)
         return p
-    def compress_range(self, data, start, length, q, lgwin, first, last, byte_align, size_hint=0, **kw):
+    def compress_range(self, data, start, length, q, lgwin, first, last, byte_align, size_hint=0, best_out=None, **kw):
         p = self.params(q, lgwin, len(data), size_hint or len(data), **kw)
         cap = length + (length >> 2) + 65536
         out = ctypes.create_string_buffer(cap)
@@ -47,7 +47,7 @@ class Model:
                                                       ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_size_t,
                                                       ctypes.POINTER(ModelStats), ctypes.c_void_p]
         n = self.lib.gpu_model_compress_range(ctypes.byref(p), data, start, length, int(first), int(last), int(byte_align), out, cap,
-                                              ctypes.byref(st), None)
+                                              ctypes.byref(st), best_out)
         return out.raw[:n], st
 
     def compress(self, data, q, lgwin, size_hint=0, best_out=None, **kw):
