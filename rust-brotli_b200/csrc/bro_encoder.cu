@@ -113,11 +113,8 @@ struct B200Encoder {
   uint32_t unit = 4096, mb_units = 1024, lcap = 64;
   int use_rle_opt = 1, split = 1, ctx_model = 1, use_dict = 1, hq_split = 1, hq_levels = HQ_MAX_LEVELS;
   uint32_t hq_unit = 0;  // parse unit of the shortest-path parse (quality >= 10); 0 = 8 KiB at q10, 16 KiB at q11 (DESIGN.md)
-  int hq_thread_units = 0;   // 1: one parse unit per thread instead of one per warp (A/B switch)
   int num_lanes = 4;
   int ondemand = 1;       // q7..q9: search deep buckets where the parse stands (1) or for every position up front (0, A/B)
-  int pair_parse = 4;     // parse units per warp for q5 / q6: 4 (default) or 2; 0 = one unit per warp (kept for A/B measurements)
-  int shallow_match = 1;  // (the loop version of the depth 16 / 32 scan is gone; the option is accepted and ignored)
   Lane lanes[kMaxLanes];
   cudaStream_t s_in = nullptr, s_out = nullptr;  // copy streams
   DevBuf d_dict_words, d_dict_hash, d_dict_lutb, d_dict_lute, d_dict_trg, d_dict_tr;
@@ -519,8 +516,7 @@ struct B200Encoder {
     // (depth >= 128 -- q8, q9 and the lgwin <= 16 configurations -- gains most on JSON logs and periodic data, where the walk
     // visits few positions; depth 64 (q7) and inputs of a few units are faster up front.  ondemand = 2 forces the on-demand path
     // for every deep configuration, 0 switches it off.)
-    const bool od_shape = P.quality < 10 && (P.depth == 64 || P.depth == 128 || P.depth == 256) && range_len <= payload_max &&
-                          (P.n_last == 4 || P.n_last == 10 || P.n_last == 16);
+    const bool od_shape = P.quality < 10 && (P.depth == 64 || P.depth == 128 || P.depth == 256) && range_len <= payload_max;
     const bool od = od_shape && (ondemand > 1 || (ondemand == 1 && P.depth >= 128 && range_len >= ((uint32_t)4 << 20)));
     DeepArgs da;
     memset(&da, 0, sizeof(da));
@@ -569,9 +565,8 @@ struct B200Encoder {
         aa.quality = P.quality;
         aa.level = 0;
         aa.last_pass = P.hq_levels == 0;
-        if (P.depth == 256) k_match_all<256><<<mgrid, MATCH_THREADS, (size_t)(MATCH_THREADS + 256) * 3 * 4, stream>>>(aa);
-        else if (P.depth == 1024) k_match_all<1024><<<mgrid, MATCH_THREADS, (size_t)(MATCH_THREADS + 1024) * 3 * 4, stream>>>(aa);
-        else { fprintf(stderr, "[brotli_b200] unsupported bucket depth %d\n", P.depth); return false; }
+        if (P.depth != 256) { fprintf(stderr, "[brotli_b200] unsupported bucket depth %d\n", P.depth); return false; }
+        k_match_all<256><<<mgrid, MATCH_THREADS, (size_t)(MATCH_THREADS + 256) * 3 * 4, stream>>>(aa);
         for (int lv = 0; lv < P.hq_levels; ++lv) {  // long-prefix levels: the batch re-sorted by the level's hash, lists merged
           run_sort<true>(L, d_all + origin, count, BRO_HASH_LEVEL0 + lv, P.key_bits);
           aa.level = lv;
@@ -600,30 +595,17 @@ struct B200Encoder {
       za.nodes = L.d_hq_nodes.as<ZNode>();
       za.pre = L.d_hq_pre.as<uint32_t>();
       za.scratch = L.d_hq_scratch.as<uint32_t>();
-      for (int phase = 1; phase <= (P.quality >= 11 ? 2 : 1); ++phase) {
-        if (hq_thread_units) k_zopfli<<<(W.num_units + 31) / 32, 32, 0, stream>>>(W, za, 1u, phase);
-        else k_zopfli<<<W.num_units, 32, 0, stream>>>(W, za, 32u, phase);
-      }
-    } else
-    if (od) {
+      for (int phase = 1; phase <= (P.quality >= 11 ? 2 : 1); ++phase) k_zopfli<<<W.num_units, 32, 0, stream>>>(W, za, phase);
+    } else {  // greedy / lazy parse: fill_params gives n_last 4 at depth 16 / 32 (q5, q6), 10 at 64 / 128 (q7, q8), 16 at 256
       const uint32_t pg = (W.num_units + PARSE_WARPS - 1) / PARSE_WARPS;
-#define B200_OD_LAUNCH(NLV) \
-      switch (P.depth) { \
-        case 64: k_parse_ondemand<NLV, 64><<<pg, PARSE_WARPS * 32, 0, stream>>>(W, da); break; \
-        case 128: k_parse_ondemand<NLV, 128><<<pg, PARSE_WARPS * 32, 0, stream>>>(W, da); break; \
-        default: k_parse_ondemand<NLV, 256><<<pg, PARSE_WARPS * 32, 0, stream>>>(W, da); break; \
-      }
-      if (P.n_last == 4) { B200_OD_LAUNCH(4) }
-      else if (P.n_last == 10) { B200_OD_LAUNCH(10) }
-      else { B200_OD_LAUNCH(16) }
-#undef B200_OD_LAUNCH
-    } else
-    if (pair_parse == 4 && P.n_last == 4 && P.hash_type != 9)  // four units per warp (q5, q6)
-      k_parse_pair<4><<<(W.num_units + 4 * PARSE_WARPS - 1) / (4 * PARSE_WARPS), PARSE_WARPS * 32, 0, stream>>>(W);
-    else if (pair_parse && P.n_last == 4 && P.hash_type != 9)  // two units per warp
-      k_parse_pair<2><<<(W.num_units + 2 * PARSE_WARPS - 1) / (2 * PARSE_WARPS), PARSE_WARPS * 32, 0, stream>>>(W);
-    else
-      k_parse<<<(W.num_units + PARSE_WARPS - 1) / PARSE_WARPS, PARSE_WARPS * 32, 0, stream>>>(W);
+      if (od && P.n_last == 10 && P.depth == 64) k_parse_ondemand<10, 64><<<pg, PARSE_WARPS * 32, 0, stream>>>(W, da);
+      else if (od && P.n_last == 10 && P.depth == 128) k_parse_ondemand<10, 128><<<pg, PARSE_WARPS * 32, 0, stream>>>(W, da);
+      else if (od && P.n_last == 16 && P.depth == 256) k_parse_ondemand<16, 256><<<pg, PARSE_WARPS * 32, 0, stream>>>(W, da);
+      else if (!od && P.n_last == 4) k_parse_pair<<<(W.num_units + 4 * PARSE_WARPS - 1) / (4 * PARSE_WARPS), PARSE_WARPS * 32, 0, stream>>>(W);
+      else if (!od && P.n_last == 10) k_parse<10><<<pg, PARSE_WARPS * 32, 0, stream>>>(W);
+      else if (!od && P.n_last == 16) k_parse<16><<<pg, PARSE_WARPS * 32, 0, stream>>>(W);
+      else { fprintf(stderr, "[brotli_b200] unsupported parse shape: n_last %d, bucket depth %d\n", P.n_last, P.depth); return false; }
+    }
     mark(L, B200_ST_FINALIZE);
     k_fin_count<<<W.num_mb, 1024, 0, stream>>>(W);
     k_fin_write<<<(W.num_units + PARSE_WARPS - 1) / PARSE_WARPS, PARSE_WARPS * 32, 0, stream>>>(W);
@@ -718,13 +700,10 @@ int b200_encoder_set_option(B200Encoder* e, int option, uint32_t value) {
     case B200_OPT_CTX_MODEL: e->ctx_model = (int)value; return 1;
     case B200_OPT_TIMING: e->timing = value != 0; return 1;
     case B200_OPT_DICT: e->use_dict = (int)value; return 1;
-    case B200_OPT_SHALLOW_MATCH: e->shallow_match = (int)value; return 1;
-    case B200_OPT_PAIR_PARSE: e->pair_parse = (int)value; return 1;
     case B200_OPT_ONDEMAND: e->ondemand = (int)value; return 1;
     case B200_OPT_HQ_LEVELS: e->hq_levels = value > HQ_MAX_LEVELS ? HQ_MAX_LEVELS : (int)value; return 1;
     case B200_OPT_HQ_SPLIT: e->hq_split = (int)value; return 1;
     case B200_OPT_HQ_UNIT: e->hq_unit = value; return 1;
-    case B200_OPT_HQ_THREAD_UNITS: e->hq_thread_units = (int)value; return 1;
     case B200_OPT_LANES: e->num_lanes = value < 1 ? 1 : (value > (uint32_t)kMaxLanes ? kMaxLanes : (int)value); return 1;
   }
   return 0;

@@ -360,7 +360,6 @@ struct HqUnit {  // everything UpdateNodes needs about the unit being parsed
   const uint32_t* lit_pre; // [len + 1]
   const int32_t* start_dc; // [4]
   ZNode* nodes;            // [len + 1]
-  int coop;                // device only: the whole warp runs this unit in lock step (same data in every lane) and shares the probes
 };
 BRO_HD uint32_t hq_max_distance(const HqUnit& U, uint32_t pos) {
   const uint64_t a = U.abs_base + U.ustart + pos;
@@ -433,11 +432,12 @@ BRO_HD_NOINLINE uint32_t hq_update_nodes(const HqUnit& U, uint32_t pos, const Hq
   const uint32_t ncand = bmin((uint32_t)hq_max_candidates(U.quality), hq_queue_size(Q));
 #ifdef __CUDA_ARCH__
   // Half of the sweep's instructions were the 16 distance-cache probes per start position, almost always ending at the first-byte
-  // test.  When the warp runs the unit in lock step, the (start k, cached distance j) pairs -- up
-  // to 5 x 16 at quality 11 -- are spread over the lanes, three independent rounds whose loads overlap; only the pairs that can
-  // improve on min_len - 1 go through the sequential part below, in the same order with the same test: identical nodes.
+  // test.  The (start k, cached distance j) pairs -- up to 5 x 16 at quality 11 -- are spread over the lanes, three independent
+  // rounds whose loads overlap; only the pairs that can improve on min_len - 1 go through the sequential part below, in the same
+  // order with the same test: identical nodes.  Every device caller must therefore run the unit with a full warp in lock step
+  // (same data in every lane): the probes are shared through warp ballots and shuffles.
   uint32_t coop_len0 = 0, coop_len1 = 0, coop_len2 = 0, coop_ball0 = 0, coop_ball1 = 0, coop_ball2 = 0;
-  if (U.coop) {
+  {
     const uint32_t lane = threadIdx.x & 31u;
     const uint32_t bl0 = min_len - 1;
 #pragma unroll
@@ -471,11 +471,9 @@ BRO_HD_NOINLINE uint32_t hq_update_nodes(const HqUnit& U, uint32_t pos, const Hq
 #endif
     for (int j = 0; j < 16 && best_len < max_len; ++j) {
 #ifdef __CUDA_ARCH__
-      if (U.coop) {
-        if (!coop_hits) break;
-        j = __ffs((int)coop_hits) - 1;
-        coop_hits &= coop_hits - 1u;
-      }
+      if (!coop_hits) break;
+      j = __ffs((int)coop_hits) - 1;
+      coop_hits &= coop_hits - 1u;
 #endif
       const int32_t backward_s = cache_candidate(pd.dc, j);  // kDistanceCacheIndex / Offset, mod.rs:653-655
       if (backward_s <= 0 || (uint32_t)backward_s > max_distance) continue;
@@ -483,7 +481,7 @@ BRO_HD_NOINLINE uint32_t hq_update_nodes(const HqUnit& U, uint32_t pos, const Hq
       const uint8_t* prev = cur - backward;
       if (cur[best_len] != prev[best_len]) continue;
 #ifdef __CUDA_ARCH__
-      const uint32_t len = U.coop ? __shfl_sync(0xffffffffu, coop_len, (int)coop_sh + j) : hq_lcp(prev, cur, max_len);
+      const uint32_t len = __shfl_sync(0xffffffffu, coop_len, (int)coop_sh + j);
 #else
       const uint32_t len = hq_lcp(prev, cur, max_len);
 #endif

@@ -819,149 +819,6 @@ __device__ __forceinline__ uint32_t warp_lcp_ext(const uint8_t* cur, uint32_t ba
   return max_len;
 }
 
-// Warp-cooperative form of parse_unit (bro_parse.cuh): identical results, but the last-distance probes of a window
-// of G = 32 / NL consecutive positions are issued by all lanes at once (lane = position * NL + candidate) and the
-// serial greedy / lazy decisions are then folded from registers with shuffles.  All scalar state is warp-uniform.
-template <int NL>
-__device__ __forceinline__ uint32_t parse_unit_warp(const EncParams& P, const uint8_t* data, const uint32_t* best,
-                                                    uint32_t ustart, uint32_t uend, RawCmd* out, uint32_t* tail,
-                                                    uint32_t* ncopy, bool D, int32_t* dc) {
-  constexpr int G = 32 / NL;
-  constexpr uint32_t CAPA = 8;  // bytes compared per probe in the parallel phase
-  const uint32_t FULL = 0xffffffffu;
-  const uint32_t lane = threadIdx.x & 31;
-  const uint32_t j_lane = lane / NL, i_lane = lane % NL;
-  const uint32_t htl = P.hash_type == 6 ? 8u : 4u;
-  const uint32_t window = P.quality < 9 ? 64u : 512u;
-  const int n_last = P.n_last;
-  uint32_t pos = ustart, insert_len = 0, ncmd = 0, copied = 0;
-  uint32_t arh = pos + window;
-  bool have_m = false;
-  Match m;
-  m.len = m.dist = m.score = 0;
-  int delayed = 0;
-
-  auto max_backward_at = [&](uint32_t p) -> uint32_t {
-    return (P.abs_base >= P.max_backward) ? P.max_backward : bmin(p + P.abs_base, P.max_backward);
-  };
-
-  while (have_m || pos + htl < uend) {
-    // ---------------- phase A: parallel probes for positions wbase .. wbase + G - 1 ----------------
-    const uint32_t wbase = pos;
-    uint32_t mylen = 0;
-    bool myvalid = false;
-    {
-      const uint32_t p = wbase + j_lane;
-      if ((int)i_lane < n_last && p < uend) {
-        const int32_t back = cache_candidate(dc, (int)i_lane);
-        if (back > 0 && (uint32_t)back <= max_backward_at(p)) {
-          myvalid = true;
-          const uint64_t x = ldu64(data + p) ^ ldu64(data + p - back);
-          mylen = x ? ((uint32_t)(__ffsll((long long)x) - 1) >> 3) : CAPA;
-          mylen = bmin(mylen, uend - p);
-        }
-      }
-    }
-    uint32_t mybest = 0;
-    if (lane < (uint32_t)G && wbase + lane < uend) mybest = best[wbase + lane];
-
-    // fold of one position of the window == find_match() of bro_parse.cuh
-    auto fold = [&](int j, uint32_t max_len, Match* o) -> bool {
-      const uint32_t p = wbase + (uint32_t)j;
-      uint32_t best_score = BRO_MIN_SCORE, best_len = 0, best_dist = 0;
-      bool found = false;
-      for (int i = 0; i < n_last; ++i) {
-        const int src = j * NL + i;
-        const bool v = __shfl_sync(FULL, (int)myvalid, src) != 0;
-        uint32_t len = __shfl_sync(FULL, mylen, src);
-        if (!v) continue;
-        const uint32_t back = (uint32_t)cache_candidate(dc, i);
-        len = bmin(len, max_len);
-        if (len == CAPA && max_len > CAPA) len = warp_lcp_ext(data + p, back, CAPA, max_len);
-        if (best_len < max_len && len <= best_len) continue;
-        if (len >= 3 || (len == 2 && i < 2)) {
-          const uint32_t score = score_last_distance(P.hash_type, len, (uint32_t)i);
-          if (best_score < score) { best_score = score; best_len = len; best_dist = back; found = true; }
-        }
-      }
-      const uint32_t b = __shfl_sync(FULL, mybest, j);
-      const uint32_t blen = b & 0xFFu;
-      if (b & BRO_BEST_DICT) {  // dictionary candidate of the match stage: only when nothing else matched
-        o->len = best_len; o->dist = best_dist; o->score = best_score;
-        if (!found && D) found = dict_decode(b, P.hash_type, max_len, max_backward_at(p), o);
-        return found;
-      }
-      if (blen != 0) {
-        const uint32_t bdist = b >> 8;
-        uint32_t len = bmin(blen, max_len);
-        if (blen >= P.lcap && max_len > len) len = warp_lcp_ext(data + p, bdist, len, max_len);
-        if (len >= 4) {
-          const uint32_t score = score_regular(P.hash_type, len, bdist);
-          if (best_score < score) { best_score = score; best_len = len; best_dist = bdist; found = true; }
-        }
-      }
-      o->len = best_len; o->dist = best_dist; o->score = best_score;
-      return found;
-    };
-
-    // ---------------- phase B: serial decisions over the window (warp-uniform) ----------------
-    int j = 0;
-    for (;;) {
-      if (!have_m) {
-        if (!(pos + htl < uend) || j >= G) break;
-        if (fold(j, uend - pos, &m)) {
-          have_m = true;
-          delayed = 0;
-        } else {
-          insert_len++;
-          pos++;
-          j++;
-          if (pos > arh) {
-            const uint32_t margin = bmax(htl - 1u, 4u);
-            if (pos + 16 + margin >= uend) { insert_len += uend - pos; pos = uend; }
-            else if (pos > arh + 4 * window) { insert_len += 16; pos += 16; }
-            else { insert_len += 8; pos += 8; }
-            break;  // jumped: new window
-          }
-          continue;
-        }
-      }
-      // a match m is pending at pos: lazy evaluation of pos + 1
-      if (j + 1 >= G) break;  // pos + 1 is outside this window: re-probe with the window starting at pos
-      {
-        Match m2;
-        const bool f2 = fold(j + 1, uend - pos - 1, &m2);
-        if (f2 && m2.score >= m.score + 175u) {
-          pos++;
-          insert_len++;
-          j++;
-          m = m2;
-          if (++delayed < 4 && pos + htl < uend) continue;
-        }
-      }
-      // accept m at pos
-      const uint32_t mlen = len_bytes(m.len);
-      arh = pos + 2 * mlen + window;
-      if (!len_is_dict(m.len) && (int32_t)m.dist != dc[0]) { dc[3] = dc[2]; dc[2] = dc[1]; dc[1] = dc[0]; dc[0] = (int32_t)m.dist; }
-      if (out && lane == 0) {
-        out[ncmd].insert_len = insert_len;
-        out[ncmd].copy_len = m.len;
-        out[ncmd].distance = m.dist;
-      }
-      ++ncmd;
-      insert_len = 0;
-      copied += mlen;
-      pos += mlen;
-      have_m = false;
-      break;  // the distance cache changed: new window
-    }
-  }
-  insert_len += uend - pos;
-  *tail = insert_len;
-  *ncopy = copied;
-  return ncmd;
-}
-
 // lane-local exact common-prefix length (>= start), used for the rare candidates that match the whole probe width
 __device__ __forceinline__ uint32_t lane_lcp_ext(const uint8_t* cur, uint32_t back, uint32_t start, uint32_t max_len) {
   while (start + 8 <= max_len) {
@@ -973,31 +830,24 @@ __device__ __forceinline__ uint32_t lane_lcp_ext(const uint8_t* cur, uint32_t ba
   return start;
 }
 
-// Fast path for n_last == 4 with the H5/H6 scores (q5, q6).  With penalties 0,39,43,43 (non-decreasing) the sequential
-// candidate fold of find_match() is exactly "highest score, ties to the lower cache index", so all 8 positions of a
-// window are resolved completely in parallel (4 lanes per position, 2 shuffle-max steps) and the serial greedy / lazy
-// walk only reads finished (found, len, dist, score) tuples: ballots locate the next match, shuffles fetch it.
-//
-// NL = 10 / 16 (q7..q9, incl. the H9 scores): same layout, each of the 4 lanes of a position probes candidates
-// i = lane, lane + 4, ...  The sequential fold with its "must be longer" pre-filter (find_match) reduces to: the longest
-// valid candidate wins, lowest index first; only among candidates that reach max_len does the score (i.e. the per-index
-// bonus) decide -- 135 points per byte always outweigh the bonus spread (<= 47).  That is a max over the key
-// len << 12 | (len == max_len ? bonus : 0) << 4 | (15 - i).
+// One parse unit per warp for NL = n_last = 10 / 16 (q7..q9, incl. the H9 scores): all 8 positions of a window are resolved
+// completely in parallel -- each of the 4 lanes of a position probes the cached distances i = lane, lane + 4, ..., and the
+// position's winner is the maximum of last_distance_key (2 shuffle-max steps) -- and the serial greedy / lazy walk only reads
+// finished (found, len, dist, score) tuples: ballots locate the next match, shuffles fetch it.
 template <int NL>
 __device__ __forceinline__ uint32_t parse_unit_warp4(const EncParams& P, const uint8_t* data, const uint32_t* best,
                                                      uint32_t ustart, uint32_t uend, RawCmd* out, uint32_t* tail,
                                                      uint32_t* ncopy, bool D, int32_t* dc) {
   constexpr int G = 8;
   constexpr int K = (NL + 3) / 4;  // candidates per lane
-  const int ht = NL == 4 ? 5 : P.hash_type;  // score family (5 and 6 share one)
+  const int ht = P.hash_type;
   constexpr uint32_t CAPA = 8;
   const uint32_t FULL = 0xffffffffu;
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t j_lane = lane >> 2, i_lane = lane & 3;
-  const bool il1 = (lane & 1u) != 0, il2 = (lane & 2u) != 0;
   int32_t dc0 = dc[0], dc1 = dc[1], dc2 = dc[2], dc3 = dc[3];
   const uint32_t htl = P.hash_type == 6 ? 8u : 4u;
-  const uint32_t window = (NL == 4 || P.quality < 9) ? 64u : 512u;
+  const uint32_t window = P.quality < 9 ? 64u : 512u;
   uint32_t pos = ustart, insert_len = 0, ncmd = 0, copied = 0;
   uint32_t arh = pos + window;
   bool have_m = false;
@@ -1011,83 +861,40 @@ __device__ __forceinline__ uint32_t parse_unit_warp4(const EncParams& P, const u
     const uint32_t p = wbase + j_lane;
     const bool p_ok = p < uend;
     const uint32_t maxl = p_ok ? uend - p : 0u;
-    uint32_t clen = 0, cdist = 0, key = 0;
-    if constexpr (NL == 4) {
-      if (p_ok) {
-        const int32_t back = il2 ? (il1 ? dc3 : dc2) : (il1 ? dc1 : dc0);  // selects, not branches
-        const uint32_t mb = near_start ? bmin(p + P.abs_base, P.max_backward) : P.max_backward;
-        if (back > 0 && (uint32_t)back <= mb) {
-          const uint64_t x = ldu64(data + p) ^ ldu64(data + p - back);
-          uint32_t len = x ? ((uint32_t)(__ffsll((long long)x) - 1) >> 3) : CAPA;
-          len = bmin(len, maxl);
-          if (len == CAPA && maxl > CAPA) len = lane_lcp_ext(data + p, (uint32_t)back, CAPA, maxl);
-          if (len >= 3 || (len == 2 && i_lane < 2)) {
-            const uint32_t score = score_last_distance(5, len, i_lane);
-            key = (score << 2) | (3u - i_lane);
-            clen = len;
-            cdist = (uint32_t)back;
-          }
-        }
-      }
-      {  // best of the 4 cache candidates of this position
-        uint32_t k = key;
-        k = max(k, __shfl_xor_sync(FULL, k, 1));
-        k = max(k, __shfl_xor_sync(FULL, k, 2));
-        const int src = (int)((lane & ~3u) + (3u - (k & 3u)));
-        const uint32_t wl = __shfl_sync(FULL, clen, src), wd = __shfl_sync(FULL, cdist, src);
-        key = k; clen = wl; cdist = wd;
-      }
-    } else {
-      const int32_t dca[4] = {dc0, dc1, dc2, dc3};
-      if (p_ok) {
-        const uint32_t mb = near_start ? bmin(p + P.abs_base, P.max_backward) : P.max_backward;
-        const uint64_t cw = ldu64(data + p);
+    uint32_t key = 0;
+    const int32_t dca[4] = {dc0, dc1, dc2, dc3};
+    if (p_ok) {
+      const uint32_t mb = near_start ? bmin(p + P.abs_base, P.max_backward) : P.max_backward;
+      const uint64_t cw = ldu64(data + p);
 #pragma unroll
-        for (int k = 0; k < K; ++k) {
-          const int i = (int)i_lane + 4 * k;
-          if (i < NL) {
-            const int32_t back = cache_candidate(dca, i);
-            if (back > 0 && (uint32_t)back <= mb) {
-              const uint64_t x = cw ^ ldu64(data + p - back);
-              uint32_t len = x ? ((uint32_t)(__ffsll((long long)x) - 1) >> 3) : CAPA;
-              len = bmin(len, maxl);
-              if (len == CAPA && maxl > CAPA) len = lane_lcp_ext(data + p, (uint32_t)back, CAPA, maxl);
-              if (len >= 3 || (len == 2 && i < 2)) {
-                const uint32_t bonus = len == maxl ? score_last_distance(ht, 0, (uint32_t)i) - 1880u : 0u;
-                key = max(key, ((len << 12) | (bonus << 4) | (uint32_t)(15 - i)) + 1u);
-              }
-            }
+      for (int k = 0; k < K; ++k) {
+        const int i = (int)i_lane + 4 * k;
+        if (i < NL) {
+          const int32_t back = cache_candidate(dca, i);
+          if (back > 0 && (uint32_t)back <= mb) {
+            const uint64_t x = cw ^ ldu64(data + p - back);
+            uint32_t len = x ? ((uint32_t)(__ffsll((long long)x) - 1) >> 3) : CAPA;
+            len = bmin(len, maxl);
+            if (len == CAPA && maxl > CAPA) len = lane_lcp_ext(data + p, (uint32_t)back, CAPA, maxl);
+            if (len >= 3 || (len == 2 && i < 2)) key = max(key, last_distance_key(ht, len, maxl, (uint32_t)i));
           }
         }
       }
-      key = max(key, __shfl_xor_sync(FULL, key, 1));
-      key = max(key, __shfl_xor_sync(FULL, key, 2));
-      if (key) {  // every lane of the position decodes the winner; key keeps "found", the score moves to the usual place
-        const uint32_t wi = 15u - ((key - 1u) & 15u);
-        clen = (key - 1u) >> 12;
-        cdist = (uint32_t)cache_candidate(dca, (int)wi);
-        key = score_last_distance(ht, clen, wi) << 2;
-      }
     }
-    uint32_t f_score = key ? (key >> 2) : BRO_MIN_SCORE, f_len = key ? clen : 0u, f_dist = key ? cdist : 0u;
+    key = max(key, __shfl_xor_sync(FULL, key, 1));
+    key = max(key, __shfl_xor_sync(FULL, key, 2));
+    Match f;  // every lane of the position decodes the winner
+    f.len = 0; f.dist = 0; f.score = BRO_MIN_SCORE;
+    if (key) {
+      const uint32_t wi = last_distance_key_decode(key, &f.len);
+      f.dist = (uint32_t)cache_candidate(dca, (int)wi);
+      f.score = score_last_distance(ht, f.len, wi);
+    }
     bool f_found = key != 0;
-    if (p_ok && i_lane == 0) {  // bucket candidate from the match kernel must be strictly better
-      const uint32_t b = best[p];
-      const uint32_t blen = b & 0xFFu;
-      if (b & BRO_BEST_DICT) {  // dictionary candidate of the match stage: only when the cache gave nothing
-        Match dm;
-        const uint32_t mb = near_start ? bmin(p + P.abs_base, P.max_backward) : P.max_backward;
-        if (!f_found && D && dict_decode(b, ht, maxl, mb, &dm)) { f_found = true; f_len = dm.len; f_dist = dm.dist; f_score = dm.score; }
-      } else if (blen != 0) {
-        const uint32_t bdist = b >> 8;
-        uint32_t len = bmin(blen, maxl);
-        if (blen >= P.lcap && maxl > len) len = lane_lcp_ext(data + p, bdist, len, maxl);
-        if (len >= 4) {
-          const uint32_t score = score_regular(ht, len, bdist);
-          if (f_score < score) { f_score = score; f_len = len; f_dist = bdist; f_found = true; }
-        }
-      }
-    }
+    if (p_ok && i_lane == 0)  // then the bucket candidate of the match kernel
+      f_found = take_best_candidate(best[p], ht, P.lcap, data + p, maxl, near_start ? bmin(p + P.abs_base, P.max_backward) : P.max_backward, D,
+                                    lane_lcp_ext, f_found, &f);
+    const uint32_t f_len = f.len, f_dist = f.dist, f_score = f.score;
     // lane 4*j now holds the finished result of position wbase + j
     uint32_t found8 = __ballot_sync(FULL, f_found && i_lane == 0);  // bits 0,4,8,.. -> compress to bits 0..7
     found8 = (found8 | (found8 >> 3)) & 0x03030303u;
@@ -1164,25 +971,25 @@ __device__ __forceinline__ uint32_t parse_unit_warp4(const EncParams& P, const u
   return ncmd;
 }
 
-// Two parse units per warp (q5 / q6 path): each half-warp resolves a window of 4 positions x 4 cached distances, and the
-// greedy / lazy walk is written as straight-line predicated code so that the two halves never diverge.  Every "scalar"
-// of parse_unit_warp4 is a per-half value here, held redundantly by the 16 lanes of the half.  tools/window_emul.cpp
-// checks on the CPU that this windowed formulation with G = 4 reproduces parse_range() command for command; it needs
-// only ~5 % more windows than G = 8, so a warp retires almost twice the units per instruction.
-// UPW = units per warp: 2 (half-warps, windows of 4 positions) or 4 (quarter-warps, windows of 2 positions; the emulation
-// counts 1.3x the windows of UPW = 2, each of them cheaper: one lazy step instead of three).
-template <int UPW>
+// Four parse units per warp (q5 / q6: n_last = 4, the H5/H6 scores): each quarter-warp resolves a window of G = 2 positions x 4
+// cached distances, and the greedy / lazy walk is written as straight-line predicated code so that the quarters never diverge.
+// With penalties 0,39,43,43 (non-decreasing) the sequential candidate fold of find_match() is exactly "highest score, ties to the
+// lower cache index", so a position is resolved in parallel by 4 lanes and 2 shuffle-max steps.  Every "scalar" of
+// parse_unit_warp4 is a per-unit value here, held redundantly by the 8 lanes of the unit.  tools/window_emul.cpp checks on the
+// CPU that this windowed formulation with G = 2 reproduces parse_range() command for command; it needs about 1.3x the windows of
+// G = 8 on text (1.1x - 1.7x over the test inputs), each of them cheaper (one lazy step instead of seven), and a warp retires
+// four units at once.
 __global__ void __launch_bounds__(PARSE_WARPS * 32, 10) k_parse_pair(Workspace W) {
-  constexpr int G = 8 / UPW;
-  constexpr uint32_t SUB = 32 / UPW;  // lanes per unit
+  constexpr int G = 2;           // positions per window
+  constexpr uint32_t SUB = 8;    // lanes per unit
   constexpr uint32_t CAPA = 8;
   const uint32_t FULL = 0xffffffffu;
   const uint32_t lane = threadIdx.x & 31;
-  const uint32_t hbase = lane & ~(SUB - 1u), hl = lane & (SUB - 1u);
+  const uint32_t hbase = lane & ~7u, hl = lane & 7u;
   const uint32_t j_lane = hl >> 2, i_lane = lane & 3u;
   const bool il1 = (lane & 1u) != 0, il2 = (lane & 2u) != 0;
   const uint32_t gw = blockIdx.x * PARSE_WARPS + (threadIdx.x >> 5);
-  const uint32_t u = (uint32_t)UPW * gw + lane / SUB;
+  const uint32_t u = 4u * gw + lane / SUB;
   const EncParams& P = W.P;
   const uint8_t* data = W.data;
   const uint32_t* best = W.best;
@@ -1242,25 +1049,13 @@ __global__ void __launch_bounds__(PARSE_WARPS * 32, 10) k_parse_pair(Workspace W
       const uint32_t wl = __shfl_sync(FULL, clen, src), wd = __shfl_sync(FULL, cdist, src);
       key = k; clen = wl; cdist = wd;
     }
-    uint32_t f_score = key ? (key >> 2) : BRO_MIN_SCORE, f_len = key ? clen : 0u, f_dist = key ? cdist : 0u;
+    Match f;
+    f.len = key ? clen : 0u; f.dist = key ? cdist : 0u; f.score = key ? (key >> 2) : BRO_MIN_SCORE;
     bool f_found = key != 0;
-    if (p_ok && i_lane == 0) {
-      const uint32_t b = best[p];
-      const uint32_t blen = b & 0xFFu;
-      if (b & BRO_BEST_DICT) {
-        Match dm;
-        const uint32_t mb = near_start ? bmin(p + P.abs_base, P.max_backward) : P.max_backward;
-        if (!f_found && D && dict_decode(b, 5, maxl, mb, &dm)) { f_found = true; f_len = dm.len; f_dist = dm.dist; f_score = dm.score; }
-      } else if (blen != 0) {
-        const uint32_t bdist = b >> 8;
-        uint32_t len = bmin(blen, maxl);
-        if (blen >= P.lcap && maxl > len) len = lane_lcp_ext(data + p, bdist, len, maxl);
-        if (len >= 4) {
-          const uint32_t score = score_regular(5, len, bdist);
-          if (f_score < score) { f_score = score; f_len = len; f_dist = bdist; f_found = true; }
-        }
-      }
-    }
+    if (p_ok && i_lane == 0)  // then the bucket candidate of the match kernel (scores of hash types 5 and 6 are the same)
+      f_found = take_best_candidate(best[p], 5, P.lcap, data + p, maxl, near_start ? bmin(p + P.abs_base, P.max_backward) : P.max_backward, D,
+                                    lane_lcp_ext, f_found, &f);
+    const uint32_t f_len = f.len, f_dist = f.dist, f_score = f.score;
     const uint32_t bal = __ballot_sync(FULL, f_found && i_lane == 0) >> hbase;  // bits 0, 4, .. of this unit's lanes
     uint32_t found = 0;                                                         // bit j <=> a match exists at wbase + j
 #pragma unroll
@@ -1339,12 +1134,12 @@ __global__ void __launch_bounds__(PARSE_WARPS * 32, 10) k_parse_pair(Workspace W
 // Deep buckets, searched on demand (q7..q9).  k_match_deep looks at up to 256 candidates for EVERY position, but the greedy / lazy
 // walk only ever asks for the positions it visits -- about half of them on text, a tenth on record-structured data with long
 // copies.  The reference has the same shape (FindLongestMatch runs where the parse stands, mod.rs:2376-2552); what it cannot do is
-// run 6144 walks at once.  Here one warp walks one unit exactly like parse_range(), and at every position it stands on the 32 lanes
+// run 6144 walks at once.  Here one warp walks one unit with parse_range() of bro_parse.cuh, and at every position it stands on the 32 lanes
 // search the bucket list of the sort stage: rank[p] (written by k_rank_sig into the best[] buffer) is the position's index in the
 // sorted list, the `depth` entries in front of it are its candidates, nearest first, 32 per round.  sig[] carries, in sorted order,
 // key << 17 | 17 hash bits of the entry's first four bytes, so bucket end and the four-byte filter are decided from two coalesced
 // 128-byte reads; only the surviving candidates touch their data.  The value computed for a position is exactly k_match_deep's
-// best[p], so the walk below is parse_range() / find_match() of bro_parse.cuh and the streams are identical.
+// best[p], so find_match_ondemand() is find_match() of bro_parse.cuh and the streams are identical.
 // ---------------------------------------------------------------------------------------------------
 struct DeepArgs {
   MatchArgs m;          // sorted list of the chunk's (single) batch; m.best holds the ranks
@@ -1487,12 +1282,12 @@ __device__ __forceinline__ bool find_match_ondemand(const EncParams& P, const De
   constexpr uint32_t CAPA = 8;
   const uint32_t FULL = 0xffffffffu;
   const uint32_t lane = threadIdx.x & 31;
-  const int ht = NL == 4 ? 5 : P.hash_type;
+  const int ht = P.hash_type;
   uint32_t cpos[DEPTH / 32], csig[DEPTH / 32];
   deep_fetch<DEPTH>(A, rank, cpos, csig);   // in flight while the cached distances are probed
   deep_prefetch<DEPTH>(A, rank_next);
   const uint32_t mb = (P.abs_base >= P.max_backward) ? P.max_backward : bmin(pos + P.abs_base, P.max_backward);
-  uint32_t key = 0, clen = 0;
+  uint32_t key = 0;
   if (lane < (uint32_t)NL) {
     const int32_t back = cache_candidate(dca, (int)lane);
     if (back > 0 && (uint32_t)back <= mb) {
@@ -1500,116 +1295,21 @@ __device__ __forceinline__ bool find_match_ondemand(const EncParams& P, const De
       uint32_t len = x ? ((uint32_t)(__ffsll((long long)x) - 1) >> 3) : CAPA;
       len = bmin(len, maxl);
       if (len == CAPA && maxl > CAPA) len = lane_lcp_ext(data + pos, (uint32_t)back, CAPA, maxl);
-      if (len >= 3 || (len == 2 && lane < 2)) {
-        clen = len;
-        if (NL == 4) key = (score_last_distance(5, len, lane) << 2) | (3u - lane);
-        else {
-          const uint32_t bonus = len == maxl ? score_last_distance(ht, 0, lane) - 1880u : 0u;
-          key = ((len << 12) | (bonus << 4) | (15u - lane)) + 1u;
-        }
-      }
+      if (len >= 3 || (len == 2 && lane < 2)) key = last_distance_key(ht, len, maxl, lane);
     }
   }
   key = __reduce_max_sync(FULL, key);
-  bool found = key != 0;
-  uint32_t f_len = 0, f_dist = 0, f_score = BRO_MIN_SCORE;
-  if (found) {
-    if (NL == 4) {
-      const uint32_t wi = 3u - (key & 3u);
-      f_len = __shfl_sync(FULL, clen, (int)wi);
-      f_dist = (uint32_t)cache_candidate(dca, (int)wi);
-      f_score = key >> 2;
-    } else {
-      const uint32_t wi = 15u - ((key - 1u) & 15u);
-      f_len = (key - 1u) >> 12;
-      f_dist = (uint32_t)cache_candidate(dca, (int)wi);
-      f_score = score_last_distance(ht, f_len, wi);
-    }
+  Match f;
+  f.len = 0; f.dist = 0; f.score = BRO_MIN_SCORE;
+  if (key) {
+    const uint32_t wi = last_distance_key_decode(key, &f.len);
+    f.dist = (uint32_t)cache_candidate(dca, (int)wi);
+    f.score = score_last_distance(ht, f.len, wi);
   }
   const uint32_t b = deep_best_warp<DEPTH>(A, P.abs_base + pos, rank, cpos, csig, s_back);
-  const uint32_t blen = b & 0xFFu;
-  if (b & BRO_BEST_DICT) {
-    Match dm;
-    if (!found && D && dict_decode(b, ht, maxl, mb, &dm)) { found = true; f_len = dm.len; f_dist = dm.dist; f_score = dm.score; }
-  } else if (blen != 0) {
-    const uint32_t bdist = b >> 8;
-    uint32_t len = bmin(blen, maxl);
-    if (blen >= P.lcap && maxl > len) len = warp_lcp_ext(data + pos, bdist, len, maxl);
-    if (len >= 4) {
-      const uint32_t score = score_regular(ht, len, bdist);
-      if (f_score < score) { f_score = score; f_len = len; f_dist = bdist; found = true; }
-    }
-  }
-  out->len = f_len; out->dist = f_dist; out->score = f_score;
+  const bool found = take_best_candidate(b, ht, P.lcap, data + pos, maxl, mb, D, warp_lcp_ext, key != 0, &f);
+  *out = f;
   return found;
-}
-
-template <int NL, int DEPTH>
-__device__ __forceinline__ uint32_t parse_range_ondemand(const EncParams& P, const DeepArgs& A, const uint8_t* data, uint32_t rstart,
-                                                         uint32_t rend, RawCmd* out, uint32_t* tail, uint32_t* ncopy, bool D, int32_t* dc,
-                                                         uint32_t* s_back) {
-  const uint32_t FULL = 0xffffffffu;
-  const uint32_t lane = threadIdx.x & 31;
-  const uint32_t htl = P.hash_type == 6 ? 8u : 4u;
-  const uint32_t window = P.quality < 9 ? 64u : 512u;
-  const uint32_t uend = rend;
-  uint32_t pos = rstart, insert_len = 0, ncmd = 0, copied = 0;
-  uint32_t arh = pos + window;
-  // ranks of 64 consecutive positions ride in the lanes (two registers): the walk mostly moves a few bytes at a time, and the
-  // second half is reloaded one half ahead of its use
-  uint32_t rk_base = 0x80000000u, rk0 = 0, rk1 = 0;  // (no position is that large: the first query loads)
-  auto rank_load = [&](uint32_t q) -> uint32_t { return q + lane < P.n ? __ldg(A.m.best + P.abs_base + q + lane) : 0u; };
-  auto rank_of = [&](uint32_t q) -> uint32_t {
-    uint32_t d = q - rk_base;
-    if (d >= 64u) { rk_base = q; rk0 = rank_load(q); rk1 = rank_load(q + 32u); d = 0; }
-    else if (d >= 32u) { rk_base += 32u; rk0 = rk1; rk1 = rank_load(rk_base + 32u); d -= 32u; }
-    return __shfl_sync(FULL, rk0, (int)d);
-  };
-  auto rank_peek = [&](uint32_t q) -> uint32_t {  // rank of a position inside the window (0 outside: prefetch only)
-    const uint32_t d = q - rk_base;
-    const uint32_t v0 = __shfl_sync(FULL, rk0, (int)(d & 31u)), v1 = __shfl_sync(FULL, rk1, (int)(d & 31u));
-    return d < 32u ? v0 : (d < 64u ? v1 : 0u);
-  };
-  while (pos + htl < uend) {
-    uint32_t max_len = uend - pos;
-    Match m;
-    if (find_match_ondemand<NL, DEPTH>(P, A, data, dc, pos, max_len, D, rank_of(pos), rank_peek(pos + 1), s_back, &m)) {
-      int delayed = 0;
-      max_len--;
-      for (;; max_len--) {
-        Match m2;
-        const bool f2 = find_match_ondemand<NL, DEPTH>(P, A, data, dc, pos + 1, max_len, D, rank_of(pos + 1), rank_peek(pos + 2), s_back, &m2);
-        if (f2 && m2.score >= m.score + 175u) {
-          pos++;
-          insert_len++;
-          m = m2;
-          if (++delayed < 4 && pos + htl < uend) continue;
-        }
-        break;
-      }
-      const uint32_t mlen = len_bytes(m.len);
-      arh = pos + 2 * mlen + window;
-      if (!len_is_dict(m.len) && (int32_t)m.dist != dc[0]) { dc[3] = dc[2]; dc[2] = dc[1]; dc[1] = dc[0]; dc[0] = (int32_t)m.dist; }
-      if (out && lane < 3) reinterpret_cast<uint32_t*>(out + ncmd)[lane] = lane == 0 ? insert_len : (lane == 1 ? m.len : m.dist);
-      ++ncmd;
-      insert_len = 0;
-      copied += mlen;
-      pos += mlen;
-    } else {
-      insert_len++;
-      pos++;
-      if (pos > arh) {
-        const uint32_t margin = bmax(htl - 1u, 4u);
-        if (pos + 16 + margin >= uend) { insert_len += uend - pos; pos = uend; }
-        else if (pos > arh + 4 * window) { insert_len += 16; pos += 16; }
-        else { insert_len += 8; pos += 8; }
-      }
-    }
-  }
-  insert_len += uend - pos;
-  *tail = insert_len;
-  *ncopy = copied;
-  return ncmd;
 }
 
 template <int NL, int DEPTH>
@@ -1624,9 +1324,34 @@ __global__ void __launch_bounds__(PARSE_WARPS * 32, 8) k_parse_ondemand(Workspac
   const bool warm = (u % P.mb_units) != 0 && s >= BRO_WARMUP_BYTES;
   RawCmd* const out = W.raw + (size_t)u * (P.unit / 2 + 1);
   __shared__ uint32_t s_back_all[PARSE_WARPS][256];
+  uint32_t* const s_back = s_back_all[threadIdx.x >> 5];
+  const uint32_t FULL = 0xffffffffu;
+  const uint32_t lane = threadIdx.x & 31;
   for (int phase = warm ? 0 : 1; phase < 2; ++phase) {
     const uint32_t rs = phase ? s : s - BRO_WARMUP_BYTES, re = phase ? e : s;
-    ncmd = parse_range_ondemand<NL, DEPTH>(P, A, W.data, rs, re, phase ? out : nullptr, &tail, &ncopy, D, dc, s_back_all[threadIdx.x >> 5]);
+    RawCmd* const o = phase ? out : nullptr;
+    // ranks of 64 consecutive positions ride in the lanes (two registers): the walk mostly moves a few bytes at a time, and the
+    // second half is reloaded one half ahead of its use
+    uint32_t rk_base = 0x80000000u, rk0 = 0, rk1 = 0;  // (no position is that large: the first query loads)
+    auto rank_load = [&](uint32_t q) -> uint32_t { return q + lane < P.n ? __ldg(A.m.best + P.abs_base + q + lane) : 0u; };
+    auto rank_of = [&](uint32_t q) -> uint32_t {
+      uint32_t d = q - rk_base;
+      if (d >= 64u) { rk_base = q; rk0 = rank_load(q); rk1 = rank_load(q + 32u); d = 0; }
+      else if (d >= 32u) { rk_base += 32u; rk0 = rk1; rk1 = rank_load(rk_base + 32u); d -= 32u; }
+      return __shfl_sync(FULL, rk0, (int)d);
+    };
+    auto rank_peek = [&](uint32_t q) -> uint32_t {  // rank of a position inside the window (0 outside: prefetch only)
+      const uint32_t d = q - rk_base;
+      const uint32_t v0 = __shfl_sync(FULL, rk0, (int)(d & 31u)), v1 = __shfl_sync(FULL, rk1, (int)(d & 31u));
+      return d < 32u ? v0 : (d < 64u ? v1 : 0u);
+    };
+    auto find = [&](uint32_t q, uint32_t max_len, Match* m) {
+      return find_match_ondemand<NL, DEPTH>(P, A, W.data, dc, q, max_len, D, rank_of(q), rank_peek(q + 1), s_back, m);
+    };
+    auto store = [&](uint32_t k, uint32_t ins, uint32_t len, uint32_t dist) {
+      if (o && lane < 3) reinterpret_cast<uint32_t*>(o + k)[lane] = lane == 0 ? ins : (lane == 1 ? len : dist);
+    };
+    ncmd = parse_range(P, rs, re, dc, find, store, &tail, &ncopy);
   }
   if ((threadIdx.x & 31) == 0) {
     W.unit_ncmd[u] = ncmd;
@@ -1638,8 +1363,9 @@ __global__ void __launch_bounds__(PARSE_WARPS * 32, 8) k_parse_ondemand(Workspac
 #ifndef PARSE_MIN_BLOCKS
 #define PARSE_MIN_BLOCKS 10
 #endif
+// q7..q9 with the bucket candidates of every position found up front: one parse unit per warp, NL = n_last = 10 / 16
+template <int NL>
 __global__ void __launch_bounds__(PARSE_WARPS * 32, PARSE_MIN_BLOCKS) k_parse(Workspace W) {
-  // One parse unit per warp.
   const uint32_t u = blockIdx.x * PARSE_WARPS + (threadIdx.x >> 5);
   if (u >= W.num_units) return;
   const EncParams& P = W.P;
@@ -1655,12 +1381,7 @@ __global__ void __launch_bounds__(PARSE_WARPS * 32, PARSE_MIN_BLOCKS) k_parse(Wo
   ncmd = 0;
   for (int phase = warm ? 0 : 1; phase < 2; ++phase) {
     const uint32_t rs = phase ? s : s - BRO_WARMUP_BYTES, re = phase ? e : s;
-    RawCmd* const o = phase ? out : nullptr;
-    const bool Dp = D;
-    if (P.n_last == 4 && P.hash_type != 9) ncmd = parse_unit_warp4<4>(P, W.data, W.best, rs, re, o, &tail, &ncopy, Dp, dc);
-    else if (P.n_last == 10) ncmd = parse_unit_warp4<10>(P, W.data, W.best, rs, re, o, &tail, &ncopy, Dp, dc);
-    else if (P.n_last == 16) ncmd = parse_unit_warp4<16>(P, W.data, W.best, rs, re, o, &tail, &ncopy, Dp, dc);
-    else ncmd = parse_unit_warp<16>(P, W.data, W.best, rs, re, o, &tail, &ncopy, Dp, dc);  // generic reference implementation
+    ncmd = parse_unit_warp4<NL>(P, W.data, W.best, rs, re, phase ? out : nullptr, &tail, &ncopy, D, dc);
   }
   if ((threadIdx.x & 31) == 0) {
     W.unit_ncmd[u] = ncmd;

@@ -166,12 +166,11 @@ struct ZopfliArgs {
   uint32_t* scratch;  // [num_units][HQ_SCRATCH_WORDS]
 };
 
-// lanes_per_unit = 32: one unit per warp (lane 0 runs the node sweep); 1: one unit per thread (32 units per warp; slower, kept as a
-// switch).  phase 1: warm-up cache, literal costs, shortest path with the initial cost model; at quality 11 the command statistics
-// stay in the unit's scratch.  phase 2 (quality 11 only): the statistics of the unit's HQ_STATS_SPAN window are pooled (all lanes),
-// costs from them, second shortest path.
-__global__ void __launch_bounds__(32) k_zopfli(Workspace W, ZopfliArgs Z, uint32_t lanes_per_unit, int phase) {
-  const uint32_t u = lanes_per_unit == 1 ? blockIdx.x * 32 + threadIdx.x : blockIdx.x;
+// One unit per warp (lane 0 runs the node sweep).  phase 1: warm-up cache, literal costs, shortest path with the initial cost
+// model; at quality 11 the command statistics stay in the unit's scratch.  phase 2 (quality 11 only): the statistics of the unit's
+// HQ_STATS_SPAN window are pooled (all lanes), costs from them, second shortest path.
+__global__ void __launch_bounds__(32) k_zopfli(Workspace W, ZopfliArgs Z, int phase) {
+  const uint32_t u = blockIdx.x;
   if (u >= W.num_units) return;
   const EncParams& P = W.P;
   const uint32_t s = u * P.unit, e = bmin(P.n, s + P.unit);
@@ -186,21 +185,19 @@ __global__ void __launch_bounds__(32) k_zopfli(Workspace W, ZopfliArgs Z, uint32
     const uint32_t gu = bmax(1u, HQ_STATS_SPAN / P.unit);
     const uint32_t mb_u0 = u / P.mb_units * P.mb_units;
     const uint32_t g0 = mb_u0 + (u - mb_u0) / gu * gu, g1 = bmin(bmin(W.num_units, g0 + gu), mb_u0 + P.mb_units);
-    const uint32_t step = lanes_per_unit == 1 ? 1u : 32u, first = lanes_per_unit == 1 ? 0u : threadIdx.x;
-    for (uint32_t k = first; k < HQ_STATS_WORDS; k += step) {
+    for (uint32_t k = threadIdx.x; k < HQ_STATS_WORDS; k += 32u) {
       uint32_t acc = 0;
       for (uint32_t v = g0; v < g1; ++v) acc += Z.scratch[(size_t)v * HQ_SCRATCH_WORDS + 769 + 768 + k];
       pooled[k] = acc;
     }
-    if (lanes_per_unit != 1) __syncwarp();
+    __syncwarp();
   }
-  // one unit per warp: every lane runs the node sweep on the same data (same loads, same stores: no more issue slots than one
-  // lane would take), so that the 16 distance-cache probes of UpdateNodes can be spread over the lanes (HqUnit::coop)
+  // every lane runs the node sweep on the same data (same loads, same stores: no more issue slots than one lane would take), so
+  // that the 16 distance-cache probes of UpdateNodes can be spread over the lanes (hq_update_nodes)
   uint32_t* pre = Z.pre + (size_t)u * (P.unit + 1);
   HqUnit U;
   U.data = W.data; U.ustart = s; U.len = e - s; U.abs_base = P.abs_base; U.max_backward = P.max_backward; U.quality = P.quality;
   U.model = model; U.lit_pre = pre; U.start_dc = warm_dc; U.nodes = Z.nodes + (size_t)u * (P.unit + 1);
-  U.coop = lanes_per_unit != 1;
   hq_model_initial(model, W.lut);
   RawCmd* out = W.raw + (size_t)u * (P.unit / 2 + 1);
   const bool two = P.quality >= 11;

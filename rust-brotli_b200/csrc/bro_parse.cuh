@@ -63,6 +63,20 @@ BRO_HD uint32_t score_last_distance(int hash_type, uint32_t len, uint32_t i) {
 }
 #define BRO_MIN_SCORE 2020u
 
+// Cache probes of n_last = 10 / 16 resolved in parallel (one candidate per lane or per probe).  The sequential fold of
+// find_match(), with its "must be longer" pre-filter, reduces to: the longest valid candidate wins, lowest index first; only
+// among candidates that reach max_len does the score (i.e. the per-index bonus) decide -- 135 points per byte always outweigh
+// the bonus spread (<= 47).  That is a max over this key of every valid candidate i of length len (0 = none).
+BRO_HD uint32_t last_distance_key(int hash_type, uint32_t len, uint32_t max_len, uint32_t i) {
+  const uint32_t bonus = len == max_len ? score_last_distance(hash_type, 0, i) - 1880u : 0u;
+  return ((len << 12) | (bonus << 4) | (15u - i)) + 1u;
+}
+// the winning candidate of a non-zero maximum of last_distance_key: its cache index, and its length in *len
+BRO_HD uint32_t last_distance_key_decode(uint32_t key, uint32_t* len) {
+  *len = (key - 1u) >> 12;
+  return 15u - ((key - 1u) & 15u);
+}
+
 // hash key of the bytes at p (buffer must be readable 8 bytes past p)
 BRO_HD uint32_t load32(const uint8_t* p) {
   return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
@@ -82,6 +96,10 @@ BRO_HD uint32_t lcp_bytes(const uint8_t* a, const uint8_t* b, uint32_t max_len) 
   uint32_t i = 0;
   while (i < max_len && a[i] == b[i]) ++i;
   return i;
+}
+// exact common-prefix length of cur[..] and (cur - back)[..], known to be >= start, capped at max_len
+BRO_HD uint32_t lcp_ext(const uint8_t* cur, uint32_t back, uint32_t start, uint32_t max_len) {
+  return start + lcp_bytes(cur - back + start, cur + start, max_len - start);
 }
 
 struct Match {
@@ -104,9 +122,32 @@ BRO_HD int32_t cache_candidate(const int32_t* dc, int i) {
   return (int32_t)((k & 1u) ? base + mag : base - mag);  // unsigned on purpose: no signed-overflow assumptions
 }
 
+// The match stage's candidate b = best[p] at cur = data + p, folded into *m, the result of the cache probes (found: it is a
+// match).  A dictionary candidate is taken only when nothing else was found (use_dict; it comes back with Match::len packed by
+// pack_dict_len()).  A bucket candidate is clamped to max_len, extended by ext past the match stage's cap lcap (ext = lcp_ext,
+// lane_lcp_ext or warp_lcp_ext), and taken when it scores strictly better.  Returns whether *m is a match.
+template <typename Ext>
+BRO_HD bool take_best_candidate(uint32_t b, int hash_type, uint32_t lcap, const uint8_t* cur, uint32_t max_len, uint32_t max_backward,
+                                bool use_dict, Ext ext, bool found, Match* m) {
+  if (b & BRO_BEST_DICT) {
+    Match dm;
+    if (!found && use_dict && dict_decode(b, hash_type, max_len, max_backward, &dm)) { *m = dm; return true; }
+    return found;
+  }
+  const uint32_t blen = b & 0xFFu;
+  if (blen != 0) {
+    const uint32_t bdist = b >> 8;
+    uint32_t len = bmin(blen, max_len);
+    if (blen >= lcap && max_len > len) len = ext(cur, bdist, len, max_len);
+    if (len >= 4) {
+      const uint32_t score = score_regular(hash_type, len, bdist);
+      if (m->score < score) { m->len = len; m->dist = bdist; m->score = score; return true; }
+    }
+  }
+  return found;
+}
+
 // Best match at pos: last-distance probes (serial state) combined with the precomputed bucket candidate.
-// use_dict: a dictionary candidate left in best[] by the match stage is taken when nothing else was found; it comes back
-// with Match::len packed by pack_dict_len().
 BRO_HD_NOINLINE bool find_match(const EncParams& P, const uint8_t* data, const uint32_t* best, const int32_t* dc,
                                 uint32_t pos, uint32_t max_len, Match* out, bool use_dict) {
   const uint32_t max_backward = (P.abs_base >= P.max_backward) ? P.max_backward : bmin(pos + P.abs_base, P.max_backward);
@@ -127,34 +168,17 @@ BRO_HD_NOINLINE bool find_match(const EncParams& P, const uint8_t* data, const u
       }
     }
   }
-  uint32_t b = best[pos];
-  if (b & BRO_BEST_DICT) {  // dictionary candidate: only when nothing else matched
-    out->len = best_len; out->dist = best_dist; out->score = best_score;
-    if (!found && use_dict) found = dict_decode(b, P.hash_type, max_len, max_backward, out);
-    return found;
-  }
-  uint32_t blen = b & 0xFFu;
-  if (blen != 0) {
-    uint32_t bdist = b >> 8;
-    uint32_t len = bmin(blen, max_len);
-    if (blen >= P.lcap && max_len > len) len += lcp_bytes(cur - bdist + len, cur + len, max_len - len);
-    if (len >= 4) {
-      uint32_t score = score_regular(P.hash_type, len, bdist);
-      if (best_score < score) {
-        best_score = score; best_len = len; best_dist = bdist;
-        found = true;
-      }
-    }
-  }
   out->len = best_len; out->dist = best_dist; out->score = best_score;
-  return found;
+  return take_best_candidate(best[pos], P.hash_type, P.lcap, cur, max_len, max_backward, use_dict, lcp_ext, found, out);
 }
 
-// Greedy + lazy parse of [rstart, rend) starting from the distance cache dc[4] (updated in place).  Writes commands
-// (copy_len >= 2) to out[] unless out is null, returns their number; *tail = literals after the last copy, *ncopy = total
-// bytes covered by copies.
-BRO_HD_NOINLINE uint32_t parse_range(const EncParams& P, const uint8_t* data, const uint32_t* best, uint32_t rstart,
-                                     uint32_t rend, RawCmd* out, uint32_t* tail, uint32_t* ncopy, bool D, int32_t* dc) {
+// Greedy + lazy parse of [rstart, rend) starting from the distance cache dc[4] (updated in place).  find(pos, max_len, Match*)
+// is the best match at pos (find_match() or its device forms, reading dc); store(k, insert_len, copy_len, distance) writes
+// command k (copy_len >= 2).  Returns the number of commands; *tail = literals after the last copy, *ncopy = total bytes
+// covered by copies.  The device walkers that instantiate it keep their state in registers only because it is inlined.
+template <typename Find, typename Store>
+BRO_HD uint32_t parse_range(const EncParams& P, uint32_t rstart, uint32_t rend, int32_t* dc, Find find, Store store,
+                            uint32_t* tail, uint32_t* ncopy) {
   const uint32_t hash_type_len = P.hash_type == 6 ? 8u : 4u;
   const uint32_t window = P.quality < 9 ? 64u : 512u;
   const uint32_t uend = rend;
@@ -163,12 +187,12 @@ BRO_HD_NOINLINE uint32_t parse_range(const EncParams& P, const uint8_t* data, co
   while (pos + hash_type_len < uend) {
     uint32_t max_len = uend - pos;
     Match m;
-    if (find_match(P, data, best, dc, pos, max_len, &m, D)) {
+    if (find(pos, max_len, &m)) {
       int delayed = 0;
       max_len--;
       for (;; max_len--) {
         Match m2;
-        bool f2 = find_match(P, data, best, dc, pos + 1, max_len, &m2, D);
+        bool f2 = find(pos + 1, max_len, &m2);
         if (f2 && m2.score >= m.score + 175u) {
           pos++;
           insert_len++;
@@ -182,11 +206,7 @@ BRO_HD_NOINLINE uint32_t parse_range(const EncParams& P, const uint8_t* data, co
       if (!len_is_dict(m.len) && (int32_t)m.dist != dc[0]) {  // dictionary references never enter the distance cache
         dc[3] = dc[2]; dc[2] = dc[1]; dc[1] = dc[0]; dc[0] = (int32_t)m.dist;
       }
-      if (out) {
-        out[ncmd].insert_len = insert_len;
-        out[ncmd].copy_len = m.len;
-        out[ncmd].distance = m.dist;
-      }
+      store(ncmd, insert_len, m.len, m.dist);
       ++ncmd;
       insert_len = 0;
       copied += mlen;
@@ -225,11 +245,13 @@ BRO_HD_NOINLINE uint32_t parse_range(const EncParams& P, const uint8_t* data, co
 BRO_HD_NOINLINE uint32_t parse_unit(const EncParams& P, const uint8_t* data, const uint32_t* best, uint32_t ustart,
                                     uint32_t uend, RawCmd* out, uint32_t* tail, uint32_t* ncopy) {
   int32_t dc[4] = {0x3fffffff, 0x3fffffff, 0x3fffffff, 0x3fffffff};
+  auto find = [&](uint32_t pos, uint32_t max_len, Match* m) { return find_match(P, data, best, dc, pos, max_len, m, P.use_dict != 0); };
   if ((ustart / P.unit) % P.mb_units != 0 && ustart >= BRO_WARMUP_BYTES) {
     uint32_t t2, c2;
-    parse_range(P, data, best, ustart - BRO_WARMUP_BYTES, ustart, nullptr, &t2, &c2, P.use_dict != 0, dc);
+    parse_range(P, ustart - BRO_WARMUP_BYTES, ustart, dc, find, [](uint32_t, uint32_t, uint32_t, uint32_t) {}, &t2, &c2);
   }
-  return parse_range(P, data, best, ustart, uend, out, tail, ncopy, P.use_dict != 0, dc);
+  return parse_range(P, ustart, uend, dc, find, [&](uint32_t k, uint32_t ins, uint32_t len, uint32_t dist) { out[k] = RawCmd{ins, len, dist}; },
+                     tail, ncopy);
 }
 
 }  // namespace bro

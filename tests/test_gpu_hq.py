@@ -2,7 +2,7 @@
 
 The match stage is compared position by position with a brute-force restatement of its contract (tests/hq_ref.py) and with
 the CPU model; the rest with the model's stream: every parse-unit size, the default unit bands, a size hint smaller than the
-data, small windows, ranges that start past 0, two sort batches in one chunk, and one parse unit per thread."""
+data, small windows, ranges that start past 0, and two sort batches in one chunk."""
 import contextlib
 import io
 
@@ -175,13 +175,3 @@ def test_hq_two_sort_batches_in_one_chunk(encoder, model):
     assert c == model.compress(d, 10, 24)[0]
     assert sys_decompress(c, len(d)) == d
 
-
-@pytest.mark.parametrize("q", [10, 11])
-def test_hq_one_unit_per_thread(encoder, model, q):
-    """k_zopfli with one parse unit per thread (32 units per warp, no cooperative probes) gives the model's stream."""
-    import rust_brotli_b200 as rb
-    d = golden_bytes("asyoulik.txt") + golden_bytes("alice29.txt")
-    with _option(encoder, rb._native.OPT_HQ_THREAD_UNITS, 1, 0):
-        c = encoder.compress(d, q, 22)
-    assert c == model.compress(d, q, 22)[0]
-    assert sys_decompress(c, len(d)) == d

@@ -78,10 +78,12 @@ def test_model_options(model):
         assert len(c) < len(base) * 1.03
 
 
-def test_windowed_parse_formulation_equals_sequential_spec(model):
+def test_shipped_parse_windows_equal_sequential_spec(model):
     """The parse kernels resolve a window of G positions with the distance cache of the window start and then walk it with
-    straight-line predicated code (G = 8: one unit per warp, G = 4: two units per warp).  tools/window_emul.cpp is that
-    formulation on the CPU; it must reproduce parse_range() command for command, for both window sizes."""
+    straight-line predicated code (G = 8: one unit per warp, q7..q9; G = 2: four units per warp, q5 / q6).  tools/window_emul.cpp
+    is that formulation on the CPU; it must reproduce parse_range() command for command, for both window sizes.  G = 2 needs
+    more windows than G = 8; measured on these inputs: 1.10x (compressed_file, q5..q7) to 1.71x (random_then_unicode, q9),
+    1.33x on alice29."""
     import ctypes
     import subprocess
     import numpy as np
@@ -102,10 +104,10 @@ def test_windowed_parse_formulation_equals_sequential_spec(model):
             p = model.params(q, 22, len(d), len(d))
             best = np.zeros(len(d) + 1, dtype=np.uint32)
             model.compress(d, q, 22, best_out=best.ctypes.data)
-            w4, w8 = ctypes.c_uint64(0), ctypes.c_uint64(0)
-            bad = L.window_emul_check(ctypes.byref(p), d + bytes(512), best.ctypes.data, len(d), ctypes.byref(w4), ctypes.byref(w8))
+            w2, w8 = ctypes.c_uint64(0), ctypes.c_uint64(0)
+            bad = L.window_emul_check(ctypes.byref(p), d + bytes(512), best.ctypes.data, len(d), ctypes.byref(w2), ctypes.byref(w8))
             assert bad == 0, (name, q)
-            assert w4.value <= w8.value * 1.25  # G = 4 costs few extra windows
+            assert w2.value <= w8.value * 1.75  # G = 2 costs at most 3/4 more windows
 
 
 def test_model_two_chunks_roundtrip(model):

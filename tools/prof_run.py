@@ -20,8 +20,6 @@ def main():
     enc.set_option(rb._native.OPT_TIMING, 1)
     enc.set_option(rb._native.OPT_LANES, int(os.environ.get("B200_LANES", "4")))
     enc.set_option(rb._native.OPT_DICT, int(os.environ.get("B200_DICT", "1")))
-    enc.set_option(rb._native.OPT_SHALLOW_MATCH, int(os.environ.get("B200_SHALLOW", "1")))
-    enc.set_option(rb._native.OPT_PAIR_PARSE, int(os.environ.get("B200_PAIR", "4")))
     t_in = torch.frombuffer(bytearray(d), dtype=torch.uint8).cuda()
     t_out = torch.empty(len(d) + (1 << 20), dtype=torch.uint8, device="cuda")
     for i in range(reps):

@@ -1,8 +1,8 @@
 // tools/window_emul.cpp -- TEST/DEVELOPMENT INFRASTRUCTURE.
 // Host emulation of the window-based parse kernels (fixed G positions resolved per window with the distance cache of the
 // window start, then the straight-line greedy / lazy walk).  Used to check, without a GPU, that the windowed formulation
-// with G = 4 (two parse units per warp) and G = 8 produces exactly the commands of the sequential specification
-// parse_range() of bro_parse.cuh.
+// with G = 2 (k_parse_pair: four parse units per warp) and G = 8 (parse_unit_warp4: one per warp) produces exactly the
+// commands of the sequential specification parse_range() of bro_parse.cuh.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -86,7 +86,7 @@ static uint32_t parse_range_windowed(const EncParams& P, const uint8_t* data, co
   return ncmd;
 }
 
-extern "C" int window_emul_check(const EncParams* Pin, const uint8_t* data, const uint32_t* best, uint32_t n, uint64_t* win4, uint64_t* win8) {
+extern "C" int window_emul_check(const EncParams* Pin, const uint8_t* data, const uint32_t* best, uint32_t n, uint64_t* win2, uint64_t* win8) {
   EncParams P = *Pin;
   const uint32_t CU = P.unit / 2 + 2;
   std::vector<RawCmd> a(CU), b(CU), c(CU);
@@ -96,8 +96,10 @@ extern "C" int window_emul_check(const EncParams* Pin, const uint8_t* data, cons
     int32_t d0[4] = {0x3fffffff, 0x3fffffff, 0x3fffffff, 0x3fffffff}, d1[4], d2[4];
     memcpy(d1, d0, 16); memcpy(d2, d0, 16);
     uint32_t t0, c0, t1, c1, t2, c2;
-    uint32_t n0 = parse_range(P, data, best, s, e, a.data(), &t0, &c0, P.use_dict != 0, d0);
-    uint32_t n1 = parse_range_windowed<4>(P, data, best, s, e, b.data(), &t1, &c1, P.use_dict != 0, d1, win4);
+    auto find = [&](uint32_t p, uint32_t max_len, Match* m) { return find_match(P, data, best, d0, p, max_len, m, P.use_dict != 0); };
+    auto store = [&](uint32_t k, uint32_t ins, uint32_t len, uint32_t dist) { a[k] = RawCmd{ins, len, dist}; };
+    uint32_t n0 = parse_range(P, s, e, d0, find, store, &t0, &c0);
+    uint32_t n1 = parse_range_windowed<2>(P, data, best, s, e, b.data(), &t1, &c1, P.use_dict != 0, d1, win2);
     uint32_t n2 = parse_range_windowed<8>(P, data, best, s, e, c.data(), &t2, &c2, P.use_dict != 0, d2, win8);
     if (n0 != n1 || n0 != n2 || t0 != t1 || t0 != t2 || c0 != c1 || c0 != c2 || memcmp(a.data(), b.data(), n0 * sizeof(RawCmd)) ||
         memcmp(a.data(), c.data(), n0 * sizeof(RawCmd)) || memcmp(d0, d1, 16) || memcmp(d0, d2, 16)) {
