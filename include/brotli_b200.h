@@ -142,7 +142,9 @@ void b200_encoder_destroy(B200Encoder* e);
 int b200_encoder_device(const B200Encoder* e); /* CUDA ordinal the encoder lives on */
 /* bit d set: device d compressed at least one shard of the last BrotliEncoderCompressMulti / CompressWorkPool call (diagnostic) */
 uint32_t b200_last_multi_device_mask(void);
-/* development switches (csrc/bro_encoder.h: A/B of kernel variants, stage timing, lanes); the defaults are the product configuration */
+/* encoder options (csrc/bro_encoder.h): context modelling and static dictionary on/off, stage timing, number of lanes, and the
+ * switches the tests use to reach single stages (on-demand search, quality 10 / 11 parse unit, levels and splitter); the
+ * defaults are the product configuration.  Returns 0 for an unknown option. */
 int b200_encoder_set_option(B200Encoder* e, int option, uint32_t value);
 size_t b200_max_compressed_size(size_t n);
 /* device_io: 0 = in / out are host pointers; 1 = both are device pointers on the encoder's GPU; 2 = host input, device output

@@ -10,7 +10,7 @@ LIB_PATH = os.environ.get("B200_LIB") or os.path.join(_HERE, "libbrotli_b200.so"
 
 NUM_STAGES = 7
 STAGE_NAMES = ("sort", "match", "parse", "finalize", "split", "header", "emit")
-OPT_UNIT, OPT_MB_UNITS, OPT_LCAP, OPT_RLE_OPT, OPT_SPLIT, OPT_CTX_MODEL, OPT_TIMING, OPT_LANES, OPT_DICT = 1, 2, 3, 4, 5, 6, 7, 8, 9
+OPT_CTX_MODEL, OPT_TIMING, OPT_LANES, OPT_DICT = 6, 7, 8, 9
 OPT_HQ_SPLIT, OPT_HQ_UNIT, OPT_ONDEMAND, OPT_HQ_LEVELS = 12, 13, 15, 16
 
 _lib = None

@@ -4,6 +4,7 @@
 // CPU model under tools/ that is used to check the kernels bit-for-bit).  Format constants are RFC 7932's;
 // the encoder-side semantics follow the reference (dropbox/rust-brotli) files cited at each function.
 #pragma once
+#include <math.h>
 #include <stdint.h>
 #include <stddef.h>
 
@@ -49,6 +50,11 @@ BRO_HD uint32_t log2_q16(const uint32_t* lut, uint32_t x) {
   return (s << 16) + lut[x >> s];
 }
 BRO_HD uint64_t xlog2x_q16(const uint32_t* lut, uint32_t x) { return (uint64_t)x * log2_q16(lut, x); }
+// the table itself (host; 65536 entries)
+inline void fill_log2_q16_lut(uint32_t* lut) {
+  lut[0] = 0;
+  for (uint32_t i = 1; i < 65536; ++i) lut[i] = (uint32_t)llround(log2((double)i) * 65536.0);
+}
 
 // ---------------------------------------------------------------------------------------------------
 // RFC 7932 constants

@@ -8,7 +8,6 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -84,25 +83,180 @@ struct EventPool {
 // the next one (sort, match, parse) and the host<->device copies.
 struct Lane {
   cudaStream_t stream = nullptr;
-  DevBuf d_sortA, d_sortB, d_sort_state, d_best, d_raw, d_unit, d_cmds, d_cmd_bits, d_lit_syms, d_cmd_syms, d_dist_syms,
-      d_hqm, d_hqn, d_hq_nodes, d_hq_pre, d_hq_scratch, d_bs_meta, d_bs_blockid, d_bs_signal, d_bs_hist, d_bs_icost, d_bs_first, d_bs_fmap, d_bs_bstart,
-      d_bs_bh_in, d_bs_bh_work, d_bs_u64, d_bs_u32, d_bs_nsurv, d_cm_in, d_cm_work, d_cm_u64, d_cm_u32, d_cm_nsurv, d_cm_counts, d_cm_maps, d_dist_cost, d_mb, d_split_u8, d_split_u32, d_split_counts, d_hist_lit, d_hist_cmd, d_hist_dist, d_split_codes, d_codes_u8,
-      d_codes_u16, d_hdr, d_huff_ws, d_ctxmap_ws, d_tree_ws, d_tree_bits, d_tree_nbits, d_cmd_tile, d_long_tab, d_seg_bits, d_sect_bits, d_sect_nbits;
+  DevBuf arena;     // every region of the chunk workspace (layout_chunk)
+  Workspace W{};    // the last chunk's workspace: the stage hooks read their results through it
   EventPool marks;  // timing marks: (event, stage that starts there); -1 ends the last stage
   std::vector<int> mark_stage;
   void release() {
-    DevBuf* all[] = {&d_hqm, &d_hqn, &d_hq_nodes, &d_hq_pre, &d_hq_scratch, &d_bs_meta, &d_bs_blockid, &d_bs_signal, &d_bs_hist, &d_bs_icost,
-                     &d_bs_first, &d_bs_fmap, &d_bs_bstart, &d_bs_bh_in, &d_bs_bh_work, &d_bs_u64, &d_bs_u32, &d_bs_nsurv, &d_cm_in, &d_cm_work, &d_cm_u64,
-                     &d_cm_u32, &d_cm_nsurv, &d_cm_counts, &d_cm_maps, &d_dist_cost, &d_sortA, &d_sortB, &d_sort_state, &d_best, &d_raw, &d_unit, &d_cmds, &d_cmd_bits, &d_lit_syms,
-                     &d_cmd_syms, &d_dist_syms, &d_mb, &d_split_u8, &d_split_u32, &d_split_counts, &d_hist_lit, &d_hist_cmd,
-                     &d_hist_dist, &d_split_codes, &d_codes_u8, &d_codes_u16, &d_hdr, &d_huff_ws, &d_ctxmap_ws, &d_tree_ws,
-                     &d_tree_bits, &d_tree_nbits, &d_cmd_tile, &d_long_tab, &d_seg_bits, &d_sect_bits, &d_sect_nbits};
-    for (auto* b : all) b->release();
+    arena.release();
     marks.destroy();
     if (stream) cudaStreamDestroy(stream);
     stream = nullptr;
   }
 };
+
+// Hands out the regions of a lane's workspace from one allocation.  Pass 1 (base == nullptr) only sizes the layout, pass 2
+// returns pointers into the arena.  Every region starts 256-byte aligned and is followed by a kGuard-byte gap, so that a small
+// overrun lands in the gap instead of in the next region.  No region carries data from one chunk to the next: each chunk
+// writes (or clears) a region before it reads it, so the layout may differ from chunk to chunk.
+constexpr size_t kGuard = 4096;
+struct Carve {
+  uint8_t* base;
+  size_t off = 0;
+  template <class T> T* take(size_t count) {
+    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+    off = (off + count * sizeof(T) + kGuard + 255) & ~(size_t)255;
+    return p;
+  }
+};
+
+struct SortBufs {
+  uint32_t *a, *b;  // ping-pong of the sort passes; the sorted positions land in b
+  uint32_t* state;  // digit counts, tile counters and look-back words
+};
+// sort regions for batches of up to nb positions
+SortBufs layout_sort(Carve& a, uint32_t nb) {
+  SortBufs s;
+  s.a = a.take<uint32_t>((size_t)nb + 16);  // (+ 64 bytes)
+  s.b = a.take<uint32_t>((size_t)nb + 16);
+  s.state = a.take<uint32_t>(sort_state_words((nb + SORT_TILE - 1) / SORT_TILE));
+  return s;
+}
+
+// workspaces of the quality >= 10 histogram stage (BrotliSplitBlock + context-map clustering); W's capacities are set
+void layout_hq_split(Carve& a, const EncParams& P, const Workspace& W, BsWs* B, CmWs* M) {
+  const uint32_t NM = W.num_mb;
+  const uint32_t mb_span = P.unit * P.mb_units;
+  memset(B, 0, sizeof(*B));
+  memset(M, 0, sizeof(*M));
+  B->cap[0] = mb_span; B->cap[1] = W.cmd_cap; B->cap[2] = W.cmd_cap;
+  B->maxb[0] = W.lit_blk_cap; B->maxb[1] = W.cmd_blk_cap; B->maxb[2] = W.dist_blk_cap;
+  for (int i = 0; i < 3; ++i) B->segc[i] = B->cap[i] / BS_SEG + 1;
+  B->cap_sum = B->cap[0] + B->cap[1] + B->cap[2];
+  B->maxb_sum = B->maxb[0] + B->maxb[1] + B->maxb[2];
+  B->segc_sum = B->segc[0] + B->segc[1] + B->segc[2];
+  B->dist_A = W.dist_A;
+  B->hist_stride = 100u * (256u + 704u + W.dist_A);
+  B->bh_sum = B->maxb[0] * 256 + B->maxb[1] * 704 + B->maxb[2] * W.dist_A;
+  B->nsurv_stride = std::max(B->maxb[0], std::max(B->maxb[1], B->maxb[2])) / 64 + 2;
+  const size_t nb = (size_t)NM * B->maxb_sum;
+  B->meta = a.take<BsMeta>((size_t)NM * 3);
+  B->blockid = a.take<uint8_t>((size_t)NM * B->cap_sum + 64);
+  B->signal = a.take<uint32_t>((size_t)NM * B->cap_sum * 4 + 16);  // (+ 64 bytes)
+  B->hist = a.take<uint32_t>((size_t)NM * B->hist_stride);
+  B->icost = a.take<uint32_t>((size_t)NM * B->hist_stride);
+  B->firstpos = a.take<uint32_t>((size_t)NM * 3 * 128);
+  B->fmap = a.take<uint8_t>((size_t)NM * B->segc_sum * 129);
+  B->enter = B->fmap + (size_t)NM * B->segc_sum * 128;
+  B->bstart = a.take<uint32_t>(nb + NM * 3 + 16);  // (+ 64 bytes)
+  B->bh_in = a.take<uint32_t>((size_t)NM * B->bh_sum);
+  B->bh_work = a.take<uint32_t>((size_t)NM * B->bh_sum);
+  B->ccost = a.take<uint64_t>(nb * 2);
+  B->bd = reinterpret_cast<int64_t*>(B->ccost + nb);
+  B->csize = a.take<uint32_t>(nb * 4); B->hsym = B->csize + nb; B->clusters = B->hsym + nb; B->bj = B->clusters + nb;
+  B->nsurv = a.take<uint32_t>((size_t)NM * 3 * B->nsurv_stride);
+  const size_t nc = (size_t)NM * (CM_LIT_MAX + CM_DIST_MAX);
+  const size_t hl = (size_t)NM * CM_LIT_MAX * 256, hd = (size_t)NM * CM_DIST_MAX * W.dist_A;
+  M->in_lit = a.take<uint32_t>(hl + hd); M->in_dist = M->in_lit + hl;
+  M->work_lit = a.take<uint32_t>(hl + hd); M->work_dist = M->work_lit + hl;
+  M->cost = a.take<uint64_t>(nc * 2);
+  M->bd = reinterpret_cast<int64_t*>(M->cost + nc);
+  M->size = a.take<uint32_t>(nc * 4); M->sym = M->size + nc; M->clusters = M->sym + nc; M->bj = M->clusters + nc;
+  M->nsurv = a.take<uint32_t>((size_t)NM * 2 * CM_NSURV_STRIDE);
+  M->counts = W.cm_counts;
+  M->lit_cmap = W.lit_cmap;
+  M->dist_cmap = W.dist_cmap;
+}
+
+struct ChunkBufs {  // the regions of a chunk that Workspace does not point to
+  SortBufs sort;
+  ZopfliArgs za;        // quality >= 10
+  BsWs bs;              // quality >= 10 with hq_split
+  CmWs cm;              //   "
+  uint64_t* dist_cost;  //   "   [num_mb][64] cost of every (NPOSTFIX, NDIRECT)
+};
+
+// The workspace of one chunk of c bytes: W's capacities and every region of the lane's arena.  W and X start zeroed.
+void layout_chunk(Carve& a, uint32_t c, const EncParams& P, Workspace* W, ChunkBufs* X) {
+  const uint32_t mb_span = P.unit * P.mb_units;
+  const uint32_t NU = (c + P.unit - 1) / P.unit;
+  const uint32_t NM = (NU + P.mb_units - 1) / P.mb_units;
+  const uint32_t cu = P.unit / 2 + 1;
+  const uint32_t cmd_cap = mb_span / 2 + 2;
+  const bool hq = P.quality >= 10, hq_split = hq && P.hq_split;
+  W->num_units = NU;
+  W->num_mb = NM;
+  W->cmd_cap = cmd_cap;
+  W->lit_blk_cap = mb_span / 512 + 2;
+  W->cmd_blk_cap = cmd_cap / 1024 + 2;
+  W->dist_blk_cap = cmd_cap / 512 + 2;
+  W->max_lit_trees = 256;
+  W->max_cmd_types = 256;
+  W->max_dist_types = 256;
+  W->dist_A = hq_split ? BRO_DIST_A_MAX : 64u;
+  W->hdr_cap = 384u << 10;
+  W->tile_cap = cmd_cap / 256 + 2;
+  W->long_cap = mb_span / LONG_INS + 1;
+  if (!hq) {
+    W->best = a.take<uint32_t>((size_t)c + 64);
+  } else {
+    W->hqm = a.take<HqMatch>(((size_t)c + 64) * HQ_MAXM);
+    W->hqn = a.take<uint8_t>((size_t)c + 64);
+    X->za.nodes = a.take<ZNode>((size_t)NU * (P.unit + 1));
+    X->za.pre = a.take<uint32_t>((size_t)NU * (P.unit + 1));
+    X->za.scratch = a.take<uint32_t>((size_t)NU * HQ_SCRATCH_WORDS);
+  }
+  W->raw = a.take<RawCmd>((size_t)NU * cu);
+  uint32_t* up = a.take<uint32_t>((size_t)NU * 7);  // one [7][NU] block: b200_stage_hq copies the first three rows at once
+  W->unit_ncmd = up; W->unit_tail = up + NU; W->unit_ncopy = up + 2 * (size_t)NU;
+  W->unit_cmd_off = up + 3 * (size_t)NU; W->unit_lit_off = up + 4 * (size_t)NU; W->unit_ndist = up + 5 * (size_t)NU; W->unit_dist_off = up + 6 * (size_t)NU;
+  W->cmds = a.take<GCmd>((size_t)NM * cmd_cap);
+  W->cmd_bits = a.take<uint32_t>((size_t)NM * cmd_cap);
+  W->cmd_tile = a.take<uint32_t>((size_t)NM * W->tile_cap);
+  W->long_tab = a.take<uint2>((size_t)NM * W->long_cap);
+  W->seg_bits = a.take<uint32_t>((size_t)NM * W->long_cap);
+  W->lit_syms = a.take<uint16_t>((size_t)c + 64);
+  W->cmd_syms = a.take<uint16_t>((size_t)NM * cmd_cap);
+  W->dist_syms = a.take<uint16_t>((size_t)NM * cmd_cap);
+  W->mb = a.take<MBDesc>(NM);
+  const size_t blk_total = (size_t)W->lit_blk_cap + W->cmd_blk_cap + W->dist_blk_cap;
+  uint8_t* t8 = a.take<uint8_t>((size_t)NM * blk_total);
+  W->lit_types = t8; W->cmd_types = t8 + (size_t)NM * W->lit_blk_cap; W->dist_types = W->cmd_types + (size_t)NM * W->cmd_blk_cap;
+  uint32_t* t32 = a.take<uint32_t>((size_t)NM * blk_total * 2);
+  W->lit_lengths = t32; t32 += (size_t)NM * W->lit_blk_cap;
+  W->lit_starts = t32; t32 += (size_t)NM * W->lit_blk_cap;
+  W->cmd_lengths = t32; t32 += (size_t)NM * W->cmd_blk_cap;
+  W->cmd_starts = t32; t32 += (size_t)NM * W->cmd_blk_cap;
+  W->dist_lengths = t32; t32 += (size_t)NM * W->dist_blk_cap;
+  W->dist_starts = t32;
+  W->split_counts = a.take<uint32_t>((size_t)NM * 6);
+  W->lit_hist = a.take<uint32_t>((size_t)NM * (W->max_lit_trees + 13) * 256);
+  W->cmd_hist = a.take<uint32_t>((size_t)NM * (W->max_cmd_types + 1) * 704);
+  W->dist_hist = a.take<uint32_t>((size_t)NM * (W->max_dist_types + 1) * W->dist_A);
+  W->split_codes = a.take<SplitCode>((size_t)NM * 3);
+  const size_t code_syms = (size_t)W->max_lit_trees * 256 + (size_t)W->max_cmd_types * 704 + (size_t)W->max_dist_types * W->dist_A;
+  uint8_t* c8 = a.take<uint8_t>((size_t)NM * code_syms);
+  W->lit_depth = c8; W->cmd_depth = c8 + (size_t)NM * W->max_lit_trees * 256;
+  W->dist_depth = W->cmd_depth + (size_t)NM * W->max_cmd_types * 704;
+  uint16_t* c16 = a.take<uint16_t>((size_t)NM * code_syms);
+  W->lit_code = c16; W->cmd_code = c16 + (size_t)NM * W->max_lit_trees * 256;
+  W->dist_code = W->cmd_code + (size_t)NM * W->max_cmd_types * 704;
+  W->hdr = a.take<uint8_t>((size_t)NM * W->hdr_cap);
+  W->ctxmap_ws = a.take<uint32_t>((size_t)NM * (256 * 64 + 1024));
+  W->lit_cmap = a.take<uint8_t>((size_t)NM * (CM_LIT_MAX + CM_DIST_MAX));
+  W->dist_cmap = W->lit_cmap + (size_t)NM * CM_LIT_MAX;
+  W->cm_counts = a.take<uint32_t>((size_t)NM * 2);
+  const size_t tree_cap = (size_t)W->max_lit_trees + W->max_cmd_types + W->max_dist_types;
+  W->tree_bits = a.take<uint8_t>((size_t)NM * tree_cap * TREE_SLOT_BYTES);
+  W->tree_nbits = a.take<uint32_t>((size_t)NM * tree_cap);
+  W->sect_bits = a.take<uint8_t>((size_t)NM * HDR_SECTIONS * SECT_BYTES);
+  W->sect_nbits = a.take<uint32_t>((size_t)NM * HDR_SECTIONS);
+  X->sort = layout_sort(a, (uint32_t)std::min<uint64_t>((uint64_t)c + (1ull << P.lgwin) + 4096, kBatchMax));
+  if (hq_split) {
+    layout_hq_split(a, P, *W, &X->bs, &X->cm);
+    X->dist_cost = a.take<uint64_t>((size_t)NM * 64);
+  }
+}
 
 }  // namespace
 
@@ -110,8 +264,7 @@ struct B200Encoder {
   int device = 0;
   bool ok = false;
   // configuration knobs (tests flip these)
-  uint32_t unit = 4096, mb_units = 1024, lcap = 64;
-  int use_rle_opt = 1, split = 1, ctx_model = 1, use_dict = 1, hq_split = 1, hq_levels = HQ_MAX_LEVELS;
+  int ctx_model = 1, use_dict = 1, hq_split = 1, hq_levels = HQ_MAX_LEVELS;
   uint32_t hq_unit = 0;  // parse unit of the shortest-path parse (quality >= 10); 0 = 8 KiB at q10, 16 KiB at q11 (DESIGN.md)
   int num_lanes = 4;
   int ondemand = 1;       // q7..q9: search deep buckets where the parse stands (1) or for every position up front (0, A/B)
@@ -140,8 +293,7 @@ struct B200Encoder {
     CUDA_OK(cudaStreamCreateWithFlags(&s_out, cudaStreamNonBlocking));
     if (!d_lut.ensure(65536 * 4)) return false;
     std::vector<uint32_t> lut(65536);
-    lut[0] = 0;
-    for (uint32_t i = 1; i < 65536; ++i) lut[i] = (uint32_t)llround(std::log2((double)i) * 65536.0);
+    fill_log2_q16_lut(lut.data());
     CUDA_OK(cudaMemcpy(d_lut.p, lut.data(), 65536 * 4, cudaMemcpyHostToDevice));
     if (!d_dict_words.ensure(sizeof(kDictData) + 64) || !d_dict_hash.ensure(sizeof(kDictHash))) return false;
     CUDA_OK(cudaMemset(d_dict_words.p, 0, sizeof(kDictData) + 64));
@@ -183,254 +335,48 @@ struct B200Encoder {
   }
 
   void fill_params(EncParams* P, int quality, int lgwin, uint64_t size_hint) const {
-    memset(P, 0, sizeof(*P));
-    quality = b200_effective_quality(quality);
-    if (lgwin < 10) lgwin = 10;
-    if (lgwin > 24) lgwin = 24;
-    P->quality = quality;
-    P->lgwin = lgwin;
-    uint32_t hint = size_hint > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)size_hint;
-    P->size_hint = hint;
-    // ChooseHasher, encode.rs:834-893 (H40-42 are not implemented there and fall back to H6 with default params)
-    if (quality >= 10) { P->hash_type = 5; P->key_bits = 15; P->hash_len = 4; P->depth = 256; P->n_last = 16; }  // bucket lists for k_match_all (with the long-prefix levels on, 64..1024 give the same size +-0.02 %)
-    else if (quality == 9) { P->hash_type = 9; P->key_bits = 15; P->hash_len = 4; P->depth = 256; P->n_last = 16; }
-    else if (lgwin <= 16) { P->hash_type = 6; P->key_bits = 15; P->hash_len = 5; P->depth = 256; P->n_last = 16; }
-    else if (hint > (1u << 22) && lgwin >= 19) {
-      P->hash_type = 6; P->key_bits = 15; P->hash_len = 5; P->depth = 1 << (quality - 1);
-      P->n_last = quality < 7 ? 4 : quality < 9 ? 10 : 16;
-    } else {
-      P->hash_type = 5; P->key_bits = (quality < 7 && hint <= (1u << 20)) ? 14 : 15; P->hash_len = 4;
-      P->depth = 1 << (quality - 1);
-      P->n_last = quality < 7 ? 4 : quality < 9 ? 10 : 16;
-    }
-    P->lcap = lcap;
-    P->unit = unit;
-    P->mb_units = mb_units;
-    P->max_backward = (1u << lgwin) - 16;
-    P->use_rle_opt = use_rle_opt;
-    P->split = split;
+    default_enc_params(P, quality, lgwin, size_hint > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)size_hint);
     P->ctx_model = ctx_model;
     P->use_dict = use_dict;
     P->hq_split = hq_split;
-    P->hq_levels = quality >= 10 ? hq_levels : 0;
-    P->hq_warm = 1;
-    if (quality >= 10) {  // same metablock span, larger parse units
-      const uint32_t span = P->unit * P->mb_units;
-      P->unit = bmin(hq_unit ? hq_unit : hq_default_unit(quality, hint), span);
-      P->mb_units = span / P->unit;
-      P->lcap = HQ_LCAP;
+    if (P->quality >= 10) {
+      P->hq_levels = hq_levels;
+      if (hq_unit) {  // same metablock span
+        const uint32_t span = P->unit * P->mb_units;
+        P->unit = bmin(hq_unit, span);
+        P->mb_units = span / P->unit;
+      }
     }
   }
 
-  // sort buffers of lane L for batches of up to nb positions: the ping-pong and the count / look-back state
-  bool ensure_sort(Lane& L, uint32_t nb) {
-    const uint32_t tiles = (nb + SORT_TILE - 1) / SORT_TILE;
-    return L.d_sortA.ensure((size_t)nb * 4 + 64) && L.d_sortB.ensure((size_t)nb * 4 + 64) &&
-           L.d_sort_state.ensure(sort_state_words(tiles) * 4);
-  }
-  // Enqueues on lane L the stable sort of the batch positions 0..count-1 (input bytes at `data`, 4096-byte aligned and padded)
-  // by the bucket key of `hash_type` (BRO_HASH_LEVEL0 + l: long-prefix level l); the sorted positions land in d_sortB.
+  // Enqueues on `stream` the stable sort of the batch positions 0..count-1 (input bytes at `data`, 4096-byte aligned and padded)
+  // by the bucket key of `hash_type` (BRO_HASH_LEVEL0 + l: long-prefix level l); the sorted positions land in S.b.
   // Three launches: the digit counts, then one one-sweep pass per digit.
   template <bool LEVEL>
-  void run_sort(Lane& L, const uint8_t* data, uint32_t count, int hash_type, int key_bits) {
-    cudaStream_t stream = L.stream;
+  void run_sort(cudaStream_t stream, const SortBufs& S, const uint8_t* data, uint32_t count, int hash_type, int key_bits) {
     SortArgs sa;
     sa.data = data;
     sa.count = count;
     sa.num_tiles = (count + SORT_TILE - 1) / SORT_TILE;
-    sa.state = L.d_sort_state.as<uint32_t>();
+    sa.state = S.state;
     sa.hash_type = hash_type;
     sa.key_bits = key_bits;
     // counts, tile counters and look-back words start at zero for every sort (batches and chunks follow each other on the lane)
     cudaMemsetAsync(sa.state, 0, sort_state_words(sa.num_tiles) * 4, stream);
     sa.pass = 0;
     sa.in = nullptr;
-    sa.outw = L.d_sortA.as<uint32_t>();
+    sa.outw = S.a;
     k_sort_count<LEVEL><<<std::min<uint32_t>(sa.num_tiles, (uint32_t)num_sms * 8), SORT_THREADS, 0, stream>>>(sa);
     k_sort_onesweep<LEVEL><<<sa.num_tiles, SORT_THREADS, 0, stream>>>(sa);
     sa.pass = 1;
-    sa.in = L.d_sortA.as<uint32_t>();
-    sa.outw = L.d_sortB.as<uint32_t>();
+    sa.in = S.a;
+    sa.outw = S.b;
     k_sort_onesweep<LEVEL><<<sa.num_tiles, SORT_THREADS, 0, stream>>>(sa);
     launches += 3;
   }
 
-  // device buffers of lane L for one chunk of `c` bytes
-  bool ensure_chunk(Lane& L, uint32_t c, const EncParams& P, Workspace* W) {
-    const uint32_t mb_span = P.unit * P.mb_units;
-    const uint32_t NU = (c + P.unit - 1) / P.unit;
-    const uint32_t NM = (NU + P.mb_units - 1) / P.mb_units;
-    const uint32_t cu = P.unit / 2 + 1;
-    const uint32_t cmd_cap = mb_span / 2 + 2;
-    W->num_units = NU;
-    W->num_mb = NM;
-    W->cmd_cap = cmd_cap;
-    W->lit_blk_cap = mb_span / 512 + 2;
-    W->cmd_blk_cap = cmd_cap / 1024 + 2;
-    W->dist_blk_cap = cmd_cap / 512 + 2;
-    W->max_lit_trees = P.split ? 256 : 13;
-    W->max_cmd_types = P.split ? 256 : 1;
-    W->max_dist_types = P.split ? 256 : 1;
-    W->dist_A = (P.quality >= 10 && P.hq_split) ? BRO_DIST_A_MAX : 64u;
-    W->hdr_cap = P.split ? (384u << 10) : (16u << 10);
-    const bool hq = P.quality >= 10;
-    if (!hq && !L.d_best.ensure(((size_t)c + 64) * 4)) return false;
-    if (hq) {
-      if (!L.d_hqm.ensure(((size_t)c + 64) * HQ_MAXM * sizeof(HqMatch)) || !L.d_hqn.ensure((size_t)c + 64)) return false;
-      if (!L.d_hq_nodes.ensure((size_t)NU * (P.unit + 1) * sizeof(ZNode)) || !L.d_hq_pre.ensure((size_t)NU * (P.unit + 1) * 4)) return false;
-      if (!L.d_hq_scratch.ensure((size_t)NU * HQ_SCRATCH_WORDS * 4)) return false;
-    }
-    if (!L.d_raw.ensure((size_t)NU * cu * sizeof(RawCmd))) return false;
-    if (!L.d_unit.ensure((size_t)NU * 7 * 4)) return false;
-    if (!L.d_cmds.ensure((size_t)NM * cmd_cap * sizeof(GCmd))) return false;
-    if (!L.d_cmd_bits.ensure((size_t)NM * cmd_cap * 4)) return false;
-    W->tile_cap = cmd_cap / 256 + 2;
-    if (!L.d_cmd_tile.ensure((size_t)NM * W->tile_cap * 4)) return false;
-    W->long_cap = mb_span / LONG_INS + 1;
-    if (!L.d_long_tab.ensure((size_t)NM * W->long_cap * 8) || !L.d_seg_bits.ensure((size_t)NM * W->long_cap * 4)) return false;
-    if (!L.d_lit_syms.ensure(((size_t)c + 64) * 2)) return false;
-    if (!L.d_cmd_syms.ensure((size_t)NM * cmd_cap * 2)) return false;
-    if (!L.d_dist_syms.ensure((size_t)NM * cmd_cap * 2)) return false;
-    if (!L.d_mb.ensure((size_t)NM * sizeof(MBDesc))) return false;
-    const size_t blk_total = (size_t)W->lit_blk_cap + W->cmd_blk_cap + W->dist_blk_cap;
-    if (!L.d_split_u8.ensure((size_t)NM * blk_total)) return false;
-    if (!L.d_split_u32.ensure((size_t)NM * blk_total * 2 * 4)) return false;
-    if (!L.d_split_counts.ensure((size_t)NM * 6 * 4)) return false;
-    if (!L.d_hist_lit.ensure((size_t)NM * (W->max_lit_trees + 13) * 256 * 4)) return false;
-    if (!L.d_hist_cmd.ensure((size_t)NM * (W->max_cmd_types + 1) * 704 * 4)) return false;
-    if (!L.d_hist_dist.ensure((size_t)NM * (W->max_dist_types + 1) * W->dist_A * 4)) return false;
-    if (!L.d_split_codes.ensure((size_t)NM * 3 * sizeof(SplitCode))) return false;
-    const size_t code_syms = (size_t)W->max_lit_trees * 256 + (size_t)W->max_cmd_types * 704 + (size_t)W->max_dist_types * W->dist_A;
-    if (!L.d_codes_u8.ensure((size_t)NM * code_syms)) return false;
-    if (!L.d_codes_u16.ensure((size_t)NM * code_syms * 2)) return false;
-    if (!L.d_hdr.ensure((size_t)NM * W->hdr_cap)) return false;
-    if (!L.d_huff_ws.ensure((size_t)NM * sizeof(HuffStoreWs))) return false;
-    if (!L.d_ctxmap_ws.ensure((size_t)NM * (256 * 64 + 1024) * 4)) return false;
-    if (!L.d_cm_maps.ensure((size_t)NM * (CM_LIT_MAX + CM_DIST_MAX)) || !L.d_cm_counts.ensure((size_t)NM * 2 * 4)) return false;
-    W->lit_cmap = L.d_cm_maps.as<uint8_t>();
-    W->dist_cmap = W->lit_cmap + (size_t)NM * CM_LIT_MAX;
-    W->cm_counts = L.d_cm_counts.as<uint32_t>();
-    const size_t tree_cap = (size_t)W->max_lit_trees + W->max_cmd_types + W->max_dist_types;
-    if (!L.d_tree_bits.ensure((size_t)NM * tree_cap * TREE_SLOT_BYTES)) return false;
-    if (!L.d_tree_nbits.ensure((size_t)NM * tree_cap * 4)) return false;
-    if (!L.d_sect_bits.ensure((size_t)NM * HDR_SECTIONS * SECT_BYTES) || !L.d_sect_nbits.ensure((size_t)NM * HDR_SECTIONS * 4)) return false;
-    if (!ensure_sort(L, std::min<uint64_t>((uint64_t)c + (1ull << P.lgwin) + 4096, kBatchMax))) return false;
-    // wire pointers
-    W->lut = d_lut.as<uint32_t>();
-    W->dict.words = d_dict_words.as<uint8_t>();
-    W->dict.hash = d_dict_hash.as<uint16_t>();
-    W->dict.lut_buckets = d_dict_lutb.as<uint16_t>();
-    W->dict.lut_entries = d_dict_lute.as<uint32_t>();
-    W->dict.tr_groups = d_dict_trg.as<uint8_t>();
-    W->dict.transforms = d_dict_tr.as<uint8_t>();
-    W->dict.num_tr_groups = BRO_DICT_NUM_TR_GROUPS;
-    W->best = L.d_best.as<uint32_t>();
-    W->hqm = L.d_hqm.as<HqMatch>();
-    W->hqn = L.d_hqn.as<uint8_t>();
-    W->raw = L.d_raw.as<RawCmd>();
-    uint32_t* up = L.d_unit.as<uint32_t>();
-    W->unit_ncmd = up; W->unit_tail = up + NU; W->unit_ncopy = up + 2 * (size_t)NU;
-    W->unit_cmd_off = up + 3 * (size_t)NU; W->unit_lit_off = up + 4 * (size_t)NU; W->unit_ndist = up + 5 * (size_t)NU; W->unit_dist_off = up + 6 * (size_t)NU;
-    W->cmds = L.d_cmds.as<GCmd>();
-    W->cmd_bits = L.d_cmd_bits.as<uint32_t>();
-    W->cmd_tile = L.d_cmd_tile.as<uint32_t>();
-    W->long_tab = L.d_long_tab.as<uint2>();
-    W->seg_bits = L.d_seg_bits.as<uint32_t>();
-    W->lit_syms = L.d_lit_syms.as<uint16_t>();
-    W->cmd_syms = L.d_cmd_syms.as<uint16_t>();
-    W->dist_syms = L.d_dist_syms.as<uint16_t>();
-    W->mb = L.d_mb.as<MBDesc>();
-    uint8_t* t8 = L.d_split_u8.as<uint8_t>();
-    W->lit_types = t8; W->cmd_types = t8 + (size_t)NM * W->lit_blk_cap; W->dist_types = W->cmd_types + (size_t)NM * W->cmd_blk_cap;
-    uint32_t* t32 = L.d_split_u32.as<uint32_t>();
-    W->lit_lengths = t32; t32 += (size_t)NM * W->lit_blk_cap;
-    W->lit_starts = t32; t32 += (size_t)NM * W->lit_blk_cap;
-    W->cmd_lengths = t32; t32 += (size_t)NM * W->cmd_blk_cap;
-    W->cmd_starts = t32; t32 += (size_t)NM * W->cmd_blk_cap;
-    W->dist_lengths = t32; t32 += (size_t)NM * W->dist_blk_cap;
-    W->dist_starts = t32;
-    W->split_counts = L.d_split_counts.as<uint32_t>();
-    W->lit_hist = L.d_hist_lit.as<uint32_t>(); W->cmd_hist = L.d_hist_cmd.as<uint32_t>(); W->dist_hist = L.d_hist_dist.as<uint32_t>();
-    W->split_codes = L.d_split_codes.as<SplitCode>();
-    uint8_t* c8 = L.d_codes_u8.as<uint8_t>();
-    W->lit_depth = c8; W->cmd_depth = c8 + (size_t)NM * W->max_lit_trees * 256;
-    W->dist_depth = W->cmd_depth + (size_t)NM * W->max_cmd_types * 704;
-    uint16_t* c16 = L.d_codes_u16.as<uint16_t>();
-    W->lit_code = c16; W->cmd_code = c16 + (size_t)NM * W->max_lit_trees * 256;
-    W->dist_code = W->cmd_code + (size_t)NM * W->max_cmd_types * 704;
-    W->hdr = L.d_hdr.as<uint8_t>();
-    W->huff_ws = L.d_huff_ws.as<HuffStoreWs>();
-    W->ctxmap_ws = L.d_ctxmap_ws.as<uint32_t>();
-    W->tree_ws = L.d_tree_ws.as<HuffStoreWs>();
-    W->tree_bits = L.d_tree_bits.as<uint8_t>();
-    W->tree_nbits = L.d_tree_nbits.as<uint32_t>();
-    W->sect_bits = L.d_sect_bits.as<uint8_t>();
-    W->sect_nbits = L.d_sect_nbits.as<uint32_t>();
-    W->total_bits = d_total.as<uint64_t>();
-    return true;
-  }
-
-  // workspaces of the quality >= 10 histogram stage (BrotliSplitBlock + context-map clustering) for one chunk
-  bool ensure_hq_split(Lane& L, const Workspace& W, BsWs* B, CmWs* M) {
-    const uint32_t NM = W.num_mb;
-    const uint32_t mb_span = W.P.unit * W.P.mb_units;
-    memset(B, 0, sizeof(*B));
-    memset(M, 0, sizeof(*M));
-    B->cap[0] = mb_span; B->cap[1] = W.cmd_cap; B->cap[2] = W.cmd_cap;
-    B->maxb[0] = W.lit_blk_cap; B->maxb[1] = W.cmd_blk_cap; B->maxb[2] = W.dist_blk_cap;
-    for (int i = 0; i < 3; ++i) B->segc[i] = B->cap[i] / BS_SEG + 1;
-    B->cap_sum = B->cap[0] + B->cap[1] + B->cap[2];
-    B->maxb_sum = B->maxb[0] + B->maxb[1] + B->maxb[2];
-    B->segc_sum = B->segc[0] + B->segc[1] + B->segc[2];
-    B->dist_A = W.dist_A;
-    B->hist_stride = 100u * (256u + 704u + W.dist_A);
-    B->bh_sum = B->maxb[0] * 256 + B->maxb[1] * 704 + B->maxb[2] * W.dist_A;
-    B->nsurv_stride = std::max(B->maxb[0], std::max(B->maxb[1], B->maxb[2])) / 64 + 2;
-    const size_t nb = (size_t)NM * B->maxb_sum;
-    if (!L.d_bs_meta.ensure((size_t)NM * 3 * sizeof(BsMeta)) || !L.d_bs_blockid.ensure((size_t)NM * B->cap_sum + 64) ||
-        !L.d_bs_signal.ensure((size_t)NM * B->cap_sum * 16 + 64) || !L.d_bs_hist.ensure((size_t)NM * B->hist_stride * 4) ||
-        !L.d_bs_icost.ensure((size_t)NM * B->hist_stride * 4) || !L.d_bs_first.ensure((size_t)NM * 3 * 128 * 4) ||
-        !L.d_bs_fmap.ensure((size_t)NM * B->segc_sum * 129) || !L.d_bs_bstart.ensure((nb + NM * 3) * 4 + 64) ||
-        !L.d_bs_bh_in.ensure((size_t)NM * B->bh_sum * 4) || !L.d_bs_bh_work.ensure((size_t)NM * B->bh_sum * 4) || !L.d_bs_u64.ensure(nb * 2 * 8) ||
-        !L.d_bs_u32.ensure(nb * 4 * 4) || !L.d_bs_nsurv.ensure((size_t)NM * 3 * B->nsurv_stride * 4))
-      return false;
-    B->meta = L.d_bs_meta.as<BsMeta>();
-    B->blockid = L.d_bs_blockid.as<uint8_t>();
-    B->signal = L.d_bs_signal.as<uint32_t>();
-    B->hist = L.d_bs_hist.as<uint32_t>();
-    B->icost = L.d_bs_icost.as<uint32_t>();
-    B->firstpos = L.d_bs_first.as<uint32_t>();
-    B->fmap = L.d_bs_fmap.as<uint8_t>();
-    B->enter = B->fmap + (size_t)NM * B->segc_sum * 128;
-    B->bstart = L.d_bs_bstart.as<uint32_t>();
-    B->bh_in = L.d_bs_bh_in.as<uint32_t>();
-    B->bh_work = L.d_bs_bh_work.as<uint32_t>();
-    B->ccost = L.d_bs_u64.as<uint64_t>();
-    B->bd = reinterpret_cast<int64_t*>(B->ccost + nb);
-    B->csize = L.d_bs_u32.as<uint32_t>(); B->hsym = B->csize + nb; B->clusters = B->hsym + nb; B->bj = B->clusters + nb;
-    B->nsurv = L.d_bs_nsurv.as<uint32_t>();
-    const size_t nc = (size_t)NM * (CM_LIT_MAX + CM_DIST_MAX);
-    const size_t hl = (size_t)NM * CM_LIT_MAX * 256, hd = (size_t)NM * CM_DIST_MAX * W.dist_A;
-    if (!L.d_cm_in.ensure((hl + hd) * 4) || !L.d_cm_work.ensure((hl + hd) * 4) || !L.d_cm_u64.ensure(nc * 2 * 8) || !L.d_cm_u32.ensure(nc * 4 * 4) ||
-        !L.d_cm_nsurv.ensure((size_t)NM * 2 * CM_NSURV_STRIDE * 4))
-      return false;
-    M->in_lit = L.d_cm_in.as<uint32_t>(); M->in_dist = M->in_lit + hl;
-    M->work_lit = L.d_cm_work.as<uint32_t>(); M->work_dist = M->work_lit + hl;
-    M->cost = L.d_cm_u64.as<uint64_t>();
-    M->bd = reinterpret_cast<int64_t*>(M->cost + nc);
-    M->size = L.d_cm_u32.as<uint32_t>(); M->sym = M->size + nc; M->clusters = M->sym + nc; M->bj = M->clusters + nc;
-    M->nsurv = L.d_cm_nsurv.as<uint32_t>();
-    M->counts = W.cm_counts;
-    M->lit_cmap = W.lit_cmap;
-    M->dist_cmap = W.dist_cmap;
-    return true;
-  }
   // BrotliSplitBlock + BrotliBuildMetaBlock's clustering for every metablock of the chunk (replaces k_split_greedy)
-  bool run_hq_split(Lane& L, const Workspace& W) {
-    BsWs B;
-    CmWs M;
-    if (!ensure_hq_split(L, W, &B, &M)) return false;
-    cudaStream_t st = L.stream;
+  bool run_hq_split(cudaStream_t st, const Workspace& W, const BsWs& B, const CmWs& M) {
     const uint32_t NM = W.num_mb;
     const dim3 g3(NM, 3), gx3(64, NM, 3), g2(NM, 2), gx2(64, NM, 2);
     k_bs_setup<<<g3, 128, 0, st>>>(W, B);
@@ -495,12 +441,28 @@ struct B200Encoder {
                  cudaEvent_t after_layout, cudaEvent_t layout_done) {
     cudaStream_t stream = L.stream;
     Workspace W;
+    ChunkBufs X;
     memset(&W, 0, sizeof(W));
+    memset(&X, 0, sizeof(X));
     EncParams P = Pstream;
     P.n = range_len;
     P.abs_base = range_start;
-    if (!ensure_chunk(L, range_len, P, &W)) return false;
+    // the whole workspace is in place before the chunk's first launch: growing the arena (cudaFree) waits for the device
+    Carve sizing{nullptr};
+    layout_chunk(sizing, range_len, P, &W, &X);
+    if (!L.arena.ensure(sizing.off)) return false;
+    Carve carve{L.arena.as<uint8_t>()};
+    layout_chunk(carve, range_len, P, &W, &X);
     W.P = P;
+    W.lut = d_lut.as<uint32_t>();
+    W.dict.words = d_dict_words.as<uint8_t>();
+    W.dict.hash = d_dict_hash.as<uint16_t>();
+    W.dict.lut_buckets = d_dict_lutb.as<uint16_t>();
+    W.dict.lut_entries = d_dict_lute.as<uint32_t>();
+    W.dict.tr_groups = d_dict_trg.as<uint8_t>();
+    W.dict.transforms = d_dict_tr.as<uint8_t>();
+    W.dict.num_tr_groups = BRO_DICT_NUM_TR_GROUPS;
+    W.total_bits = d_total.as<uint64_t>();
     W.data = d_data.as<uint8_t>() + (range_start - data_base);
     W.out = d_outw;
     W.out_cap_bytes = out_cap_bytes;
@@ -527,10 +489,10 @@ struct B200Encoder {
       if (origin < data_base) origin = (uint32_t)data_base;
       const uint32_t count = b1 - origin;
       mark(L, B200_ST_SORT);
-      run_sort<false>(L, d_all + origin, count, P.hash_type, P.key_bits);
+      run_sort<false>(stream, X.sort, d_all + origin, count, P.hash_type, P.key_bits);
       MatchArgs ma;
       ma.data = d_all;
-      ma.sorted = L.d_sortB.as<uint32_t>();
+      ma.sorted = X.sort.b;
       ma.count = count;
       ma.origin = origin;
       ma.payload_begin = (uint32_t)b0 - origin;
@@ -548,8 +510,8 @@ struct B200Encoder {
       const uint32_t mgrid = (count + MATCH_THREADS - 1) / MATCH_THREADS;
       if (od) {  // ranks into best[], signatures into the free half of the sort ping-pong
         da.m = ma;
-        da.sig = L.d_sortA.as<uint32_t>();
-        k_rank_sig<<<(count + 255) / 256, 256, 0, stream>>>(ma, L.d_sortA.as<uint32_t>());
+        da.sig = X.sort.a;
+        k_rank_sig<<<(count + 255) / 256, 256, 0, stream>>>(ma, X.sort.a);
         if (od_probe) {  // stage hook only: the search of every position, while the ranks and signatures are intact
           const uint32_t pg = (range_len + 7) / 8;
           if (P.depth == 64) k_od_probe<64><<<pg, 256, 0, stream>>>(da, range_start, range_len, od_probe);
@@ -568,7 +530,7 @@ struct B200Encoder {
         if (P.depth != 256) { fprintf(stderr, "[brotli_b200] unsupported bucket depth %d\n", P.depth); return false; }
         k_match_all<256><<<mgrid, MATCH_THREADS, (size_t)(MATCH_THREADS + 256) * 3 * 4, stream>>>(aa);
         for (int lv = 0; lv < P.hq_levels; ++lv) {  // long-prefix levels: the batch re-sorted by the level's hash, lists merged
-          run_sort<true>(L, d_all + origin, count, BRO_HASH_LEVEL0 + lv, P.key_bits);
+          run_sort<true>(stream, X.sort, d_all + origin, count, BRO_HASH_LEVEL0 + lv, P.key_bits);
           aa.level = lv;
           aa.last_pass = lv + 1 == P.hq_levels;
           k_match_level<HQ_LEVEL_DEPTH><<<mgrid, MATCH_THREADS, (size_t)(MATCH_THREADS + HQ_LEVEL_DEPTH) * 3 * 4, stream>>>(aa);
@@ -591,11 +553,7 @@ struct B200Encoder {
     }
     mark(L, B200_ST_PARSE);
     if (P.quality >= 10) {  // shortest-path parse, one unit per warp
-      ZopfliArgs za;
-      za.nodes = L.d_hq_nodes.as<ZNode>();
-      za.pre = L.d_hq_pre.as<uint32_t>();
-      za.scratch = L.d_hq_scratch.as<uint32_t>();
-      for (int phase = 1; phase <= (P.quality >= 11 ? 2 : 1); ++phase) k_zopfli<<<W.num_units, 32, 0, stream>>>(W, za, phase);
+      for (int phase = 1; phase <= (P.quality >= 11 ? 2 : 1); ++phase) k_zopfli<<<W.num_units, 32, 0, stream>>>(W, X.za, phase);
     } else {  // greedy / lazy parse: fill_params gives n_last 4 at depth 16 / 32 (q5, q6), 10 at 64 / 128 (q7, q8), 16 at 256
       const uint32_t pg = (W.num_units + PARSE_WARPS - 1) / PARSE_WARPS;
       if (od && P.n_last == 10 && P.depth == 64) k_parse_ondemand<10, 64><<<pg, PARSE_WARPS * 32, 0, stream>>>(W, da);
@@ -611,9 +569,8 @@ struct B200Encoder {
     k_fin_write<<<(W.num_units + PARSE_WARPS - 1) / PARSE_WARPS, PARSE_WARPS * 32, 0, stream>>>(W);
     k_fin_dist<<<W.num_mb, 1024, 0, stream>>>(W);
     if (P.quality >= 10 && P.hq_split) {  // NPOSTFIX / NDIRECT of every metablock (metablock.rs:152-207), commands re-coded
-      if (!L.d_dist_cost.ensure((size_t)W.num_mb * 64 * 8)) return false;
-      k_dist_cost<<<dim3(64, W.num_mb), 256, 0, stream>>>(W, L.d_dist_cost.as<uint64_t>());
-      k_dist_apply<<<dim3(64, W.num_mb), 256, 0, stream>>>(W, L.d_dist_cost.as<uint64_t>());
+      k_dist_cost<<<dim3(64, W.num_mb), 256, 0, stream>>>(W, X.dist_cost);
+      k_dist_apply<<<dim3(64, W.num_mb), 256, 0, stream>>>(W, X.dist_cost);
       launches += 2;
     }
     {
@@ -625,9 +582,8 @@ struct B200Encoder {
     mark(L, B200_ST_SPLIT);
     {
       dim3 g(W.num_mb, 3);
-      if (P.quality >= 10 && P.hq_split) { if (!run_hq_split(L, W)) return false; }
-      else if (P.split) k_split_greedy<<<g, SPLIT_THREADS, SPLIT_SMEM_WORDS * 4, stream>>>(W);
-      else k_split_simple<<<g, 512, 0, stream>>>(W);
+      if (P.quality >= 10 && P.hq_split) { if (!run_hq_split(stream, W, X.bs, X.cm)) return false; }
+      else k_split_greedy<<<g, SPLIT_THREADS, SPLIT_SMEM_WORDS * 4, stream>>>(W);
     }
     mark(L, B200_ST_HEADER);
     {
@@ -652,6 +608,7 @@ struct B200Encoder {
     }
     mark(L, -1);
     launches += 19;
+    L.W = W;
     CUDA_OK(cudaGetLastError());
     return true;
   }
@@ -667,13 +624,8 @@ int b200_device_count(void) {
   if (cudaGetDeviceCount(&n) != cudaSuccess) return 0;
   return n;
 }
-// The quality the device path runs for a requested one: 5..9 hash-chain family (encode.rs:834-893), 10 / 11 shortest-path parse;
-// q0..q4 (BasicHasher H2..H54, fragment compressors) are not built and run as 5.
-int b200_effective_quality(int requested_quality) {
-  if (requested_quality < 5) return 5;
-  if (requested_quality > 11) return 11;
-  return requested_quality;
-}
+// The quality the device path runs for a requested one (bro_parse.cuh: effective_quality)
+int b200_effective_quality(int requested_quality) { return effective_quality(requested_quality); }
 
 B200Encoder* b200_encoder_create(int device) {
   B200Encoder* e = new B200Encoder();
@@ -692,11 +644,6 @@ void b200_encoder_destroy(B200Encoder* e) {
 int b200_encoder_set_option(B200Encoder* e, int option, uint32_t value) {
   if (!e) return 0;
   switch (option) {
-    case B200_OPT_UNIT: e->unit = value; return 1;
-    case B200_OPT_MB_UNITS: e->mb_units = value; return 1;
-    case B200_OPT_LCAP: e->lcap = value > 255 ? 255 : value; return 1;
-    case B200_OPT_RLE_OPT: e->use_rle_opt = (int)value; return 1;
-    case B200_OPT_SPLIT: e->split = (int)value; return 1;
     case B200_OPT_CTX_MODEL: e->ctx_model = (int)value; return 1;
     case B200_OPT_TIMING: e->timing = value != 0; return 1;
     case B200_OPT_DICT: e->use_dict = (int)value; return 1;
@@ -861,7 +808,7 @@ int b200_stage_match(B200Encoder* e, int quality, int lgwin, uint64_t size_hint,
     cudaDeviceSynchronize();
     return 0;
   }
-  const void* src = search ? e->d_probe.p : e->lanes[0].d_best.p;
+  const void* src = search ? e->d_probe.p : (const void*)e->lanes[0].W.best;
   return cudaMemcpy(best_out, src, range_len * 4, cudaMemcpyDeviceToHost) == cudaSuccess;
 }
 
@@ -875,14 +822,12 @@ int b200_stage_hq(B200Encoder* e, int quality, int lgwin, const uint8_t* in, siz
     cudaDeviceSynchronize();
     return 0;
   }
-  EncParams P;
-  e->fill_params(&P, quality, lgwin, n);
-  const uint32_t nu = (uint32_t)((n + P.unit - 1) / P.unit);
-  Lane& L = e->lanes[0];
-  bool ok = cudaMemcpy(hqn, L.d_hqn.p, n, cudaMemcpyDeviceToHost) == cudaSuccess;
-  ok = ok && cudaMemcpy(hqm, L.d_hqm.p, n * HQ_MAXM * 8, cudaMemcpyDeviceToHost) == cudaSuccess;
-  ok = ok && cudaMemcpy(units, L.d_unit.p, (size_t)nu * 3 * 4, cudaMemcpyDeviceToHost) == cudaSuccess;
-  ok = ok && cudaMemcpy(raw, L.d_raw.p, (size_t)nu * (P.unit / 2 + 1) * 12, cudaMemcpyDeviceToHost) == cudaSuccess;
+  const Workspace& W = e->lanes[0].W;
+  const uint32_t nu = W.num_units;
+  bool ok = cudaMemcpy(hqn, W.hqn, n, cudaMemcpyDeviceToHost) == cudaSuccess;
+  ok = ok && cudaMemcpy(hqm, W.hqm, n * HQ_MAXM * 8, cudaMemcpyDeviceToHost) == cudaSuccess;
+  ok = ok && cudaMemcpy(units, W.unit_ncmd, (size_t)nu * 3 * 4, cudaMemcpyDeviceToHost) == cudaSuccess;  // ncmd, tail, ncopy
+  ok = ok && cudaMemcpy(raw, W.raw, (size_t)nu * (W.P.unit / 2 + 1) * 12, cudaMemcpyDeviceToHost) == cudaSuccess;
   return ok ? 1 : 0;
 }
 
@@ -894,16 +839,20 @@ int b200_stage_sort(B200Encoder* e, int quality, int lgwin, const uint8_t* in, s
   EncParams P;
   e->fill_params(&P, quality, lgwin, n);
   Lane& L = e->lanes[0];
-  if (!e->d_data.ensure(n + kPad) || !e->ensure_sort(L, (uint32_t)n)) return 0;
+  Carve sizing{nullptr};
+  layout_sort(sizing, (uint32_t)n);
+  if (!e->d_data.ensure(n + kPad) || !L.arena.ensure(sizing.off)) return 0;
+  Carve carve{L.arena.as<uint8_t>()};
+  const SortBufs S = layout_sort(carve, (uint32_t)n);
   e->data_base = 0;
   uint8_t* dd = e->d_data.as<uint8_t>();
   bool ok = cudaMemcpyAsync(dd, in, n, cudaMemcpyHostToDevice, L.stream) == cudaSuccess &&
             cudaMemsetAsync(dd + n, 0, kPad, L.stream) == cudaSuccess;
   if (!ok) return 0;
-  if (level < 0) e->run_sort<false>(L, dd, (uint32_t)n, P.hash_type, P.key_bits);
-  else e->run_sort<true>(L, dd, (uint32_t)n, BRO_HASH_LEVEL0 + level, P.key_bits);
+  if (level < 0) e->run_sort<false>(L.stream, S, dd, (uint32_t)n, P.hash_type, P.key_bits);
+  else e->run_sort<true>(L.stream, S, dd, (uint32_t)n, BRO_HASH_LEVEL0 + level, P.key_bits);
   ok = cudaStreamSynchronize(L.stream) == cudaSuccess;
-  return ok && cudaMemcpy(sorted_out, L.d_sortB.p, n * 4, cudaMemcpyDeviceToHost) == cudaSuccess;
+  return ok && cudaMemcpy(sorted_out, S.b, n * 4, cudaMemcpyDeviceToHost) == cudaSuccess;
 }
 
 // parse unit the quality >= 10 path uses for this size hint with the encoder's current options (sizes the b200_stage_hq buffers)

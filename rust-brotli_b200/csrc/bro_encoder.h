@@ -6,8 +6,7 @@
 extern "C" {
 #endif
 typedef struct B200Encoder B200Encoder;
-enum { B200_OPT_UNIT = 1, B200_OPT_MB_UNITS = 2, B200_OPT_LCAP = 3, B200_OPT_RLE_OPT = 4, B200_OPT_SPLIT = 5,
-       B200_OPT_CTX_MODEL = 6, B200_OPT_TIMING = 7, B200_OPT_LANES = 8, B200_OPT_DICT = 9, B200_OPT_HQ_SPLIT = 12, B200_OPT_HQ_UNIT = 13, B200_OPT_ONDEMAND = 15, B200_OPT_HQ_LEVELS = 16 };
+enum { B200_OPT_CTX_MODEL = 6, B200_OPT_TIMING = 7, B200_OPT_LANES = 8, B200_OPT_DICT = 9, B200_OPT_HQ_SPLIT = 12, B200_OPT_HQ_UNIT = 13, B200_OPT_ONDEMAND = 15, B200_OPT_HQ_LEVELS = 16 };
 /* stage timing slots of b200_encoder_last_timings */
 enum { B200_ST_SORT = 0, B200_ST_MATCH = 1, B200_ST_PARSE = 2, B200_ST_FINALIZE = 3, B200_ST_SPLIT = 4, B200_ST_HEADER = 5,
        B200_ST_EMIT = 6, B200_NUM_STAGES = 7 };

@@ -620,6 +620,42 @@ BRO_HD uint32_t hq_default_unit(int quality, uint32_t size_hint) {
   return quality >= 11 ? 16384u : 8192u;
 }
 
+// Default parameters of a (quality, lgwin, size hint) configuration, shared by the device encoder and its CPU model.  P->n and
+// P->abs_base are left 0: they describe the range being compressed.  size_hint = 0 means unknown.
+inline void default_enc_params(EncParams* P, int quality, int lgwin, uint32_t size_hint) {
+  *P = EncParams{};
+  quality = effective_quality(quality);
+  lgwin = lgwin < 10 ? 10 : (lgwin > 24 ? 24 : lgwin);
+  P->quality = quality;
+  P->lgwin = lgwin;
+  P->size_hint = size_hint;
+  // ChooseHasher, encode.rs:834-893 (H40-42 are not implemented there and fall back to H6 with default params)
+  if (quality >= 10) { P->hash_type = 5; P->key_bits = 15; P->hash_len = 4; P->depth = 256; P->n_last = 16; }  // bucket lists for k_match_all (with the long-prefix levels on, 64..1024 give the same size +-0.02 %)
+  else if (quality == 9) { P->hash_type = 9; P->key_bits = 15; P->hash_len = 4; P->depth = 256; P->n_last = 16; }
+  else if (lgwin <= 16) { P->hash_type = 6; P->key_bits = 15; P->hash_len = 5; P->depth = 256; P->n_last = 16; }
+  else if (size_hint > (1u << 22) && lgwin >= 19) {
+    P->hash_type = 6; P->key_bits = 15; P->hash_len = 5; P->depth = 1 << (quality - 1);
+    P->n_last = quality < 7 ? 4 : quality < 9 ? 10 : 16;
+  } else {
+    P->hash_type = 5; P->key_bits = (quality < 7 && size_hint <= (1u << 20)) ? 14 : 15; P->hash_len = 4;
+    P->depth = 1 << (quality - 1);
+    P->n_last = quality < 7 ? 4 : quality < 9 ? 10 : 16;
+  }
+  P->lcap = 64;
+  P->unit = 4096;
+  P->mb_units = 1024;  // 4 MiB metablocks
+  if (quality >= 10) {  // same metablock span, larger parse units
+    P->lcap = HQ_LCAP;
+    P->unit = hq_default_unit(quality, size_hint);
+    P->mb_units = (4u << 20) / P->unit;
+  }
+  P->max_backward = (1u << lgwin) - 16;
+  P->ctx_model = 1;
+  P->use_dict = 1;
+  P->hq_split = 1;
+  P->hq_levels = quality >= 10 ? HQ_MAX_LEVELS : 0;
+}
+
 // Quality 11 runs the shortest path twice, the second time with costs taken from the commands of the first pass
 // (set_from_commands, hq.rs:1076-1154).  The reference has one 256 KiB block to take them from; a 8 KiB parse unit alone is too
 // small a sample (+0.7 % on text against +0.37 % for 64 KiB units), so the statistics of the first pass are pooled over the units

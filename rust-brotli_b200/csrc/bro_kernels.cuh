@@ -3,13 +3,13 @@
 // Stage map (DESIGN.md has the data layout and the per-kernel roofline):
 //   sort    k_sort_count / k_sort_onesweep (x2)   stable one-sweep LSD radix sort of positions by bucket key
 //                                                 (replaces hasher Store*)
-//   match   k_match          every position vs the `depth` most recent earlier positions of its bucket
+//   match   k_match_shallow / k_match_deep   every position vs the `depth` most recent earlier positions of its bucket
 //                            (replaces the bucket walk of FindLongestMatch, backward_references/mod.rs:1754-1792)
 //   parse   k_parse          greedy+lazy parse per unit (CreateBackwardReferences mod.rs:2376)
 //   final   k_fin_count / k_fin_write / k_fin_dist    command records, literal/distance ranks
 //   ctx     k_ctx_decide     literal context map choice (encode.rs:1873)
 //   syms    k_symbols        symbol streams for the splitter
-//   split   k_split_simple / k_split_greedy           histograms + greedy block split (metablock.rs:551-1021)
+//   split   k_split_greedy   histograms + greedy block split (metablock.rs:551-1021)
 //   header  k_header         Huffman codes + metablock header bits (brotli_bit_stream.rs:2035-2190)
 //   emit    k_bitlen / k_bitscan / k_layout / k_emit_header / k_emit_body / k_emit_raw
 #pragma once
@@ -98,8 +98,6 @@ struct Workspace {
   // header
   uint8_t* hdr;           // [num_mb][hdr_cap]
   uint32_t hdr_cap;
-  HuffStoreWs* huff_ws;   // [num_mb]
-  HuffStoreWs* tree_ws;   // [num_mb][tree_cap]
   uint8_t* tree_bits;     // [num_mb][tree_cap][TREE_SLOT_BYTES]
   uint32_t* tree_nbits;   // [num_mb][tree_cap]
   uint8_t* sect_bits;     // [num_mb][HDR_SECTIONS][SECT_BYTES] header sections built beside the trees
@@ -1760,7 +1758,6 @@ __global__ void __launch_bounds__(256) k_symbols(Workspace W) {
 
 // ---------------------------------------------------------------------------------------------------
 // Histograms / block split.  grid = (num_mb, 3 categories).
-// k_split_simple: one block type per category (split disabled).
 // ---------------------------------------------------------------------------------------------------
 struct CatInfo {
   const uint16_t* syms;
@@ -1793,29 +1790,6 @@ __device__ __forceinline__ CatInfo cat_info(const Workspace& W, uint32_t m, int 
   if (c.max_types > (cat == 0 ? W.max_lit_trees / c.nctx : (cat == 1 ? W.max_cmd_types : W.max_dist_types)))
     c.max_types = (cat == 0 ? W.max_lit_trees / c.nctx : (cat == 1 ? W.max_cmd_types : W.max_dist_types));
   return c;
-}
-
-__global__ void __launch_bounds__(512) k_split_simple(Workspace W) {
-  __shared__ uint32_t sh[13 * 256];
-  const uint32_t m = blockIdx.x;
-  const CatInfo c = cat_info(W, m, (int)blockIdx.y);
-  const uint32_t HA = c.nctx * c.A;
-  for (uint32_t i = threadIdx.x; i < HA; i += blockDim.x) sh[i] = 0;
-  __syncthreads();
-  for (uint32_t i = threadIdx.x; i < c.count; i += blockDim.x) {
-    uint32_t s = c.syms[i];
-    uint32_t sym = c.nctx == 1 ? s : (s & 0xFFu) + (s >> 8) * c.A;
-    atomicAdd(&sh[sym], 1u);
-  }
-  __syncthreads();
-  for (uint32_t i = threadIdx.x; i < HA; i += blockDim.x) c.hist[i] = sh[i];
-  if (threadIdx.x == 0) {
-    c.types[0] = 0;
-    c.lengths[0] = c.count < c.min_block ? c.min_block : c.count;
-    c.starts[0] = 0;
-    c.counts[0] = 1;
-    c.counts[1] = 1;
-  }
 }
 
 // Greedy splitter: one CTA per (metablock, category); the symbol stream is consumed block by block, histograms
@@ -2025,7 +1999,6 @@ __global__ void __launch_bounds__(32) k_trees(Workspace W) {
   const uint32_t m = blockIdx.y;
   const uint32_t lane = threadIdx.x;
   const MBDesc& mb = W.mb[m];
-  const EncParams& P = W.P;
   const uint32_t nctx = ctxmap_num_contexts(mb.ctx_map_id);
   const uint32_t* cnt = W.split_counts + (size_t)m * 6;
   const bool full = mb.ctx_map_id >= CTXMAP_FULL_UTF8;  // quality >= 10: codes = clusters of the context maps
@@ -2073,7 +2046,7 @@ __global__ void __launch_bounds__(32) k_trees(Workspace W) {
   // smoothing scan and the run-length coding are chains of dependent accesses ==
   for (uint32_t i = lane; i < A; i += 32) { s_hist[i] = hist[i]; s_depth[i] = 0; s_code[i] = 0; }
   __syncwarp();
-  if (P.use_rle_opt && lane == 0) huff_smooth_counts(A, s_hist);
+  if (lane == 0) huff_smooth_counts(A, s_hist);
   __syncwarp();
   uint32_t max_bits = 0;
   for (uint32_t c = (alphabet ? alphabet : A) - 1; c; c >>= 1) ++max_bits;

@@ -205,7 +205,7 @@ __global__ void __launch_bounds__(32) k_zopfli(Workspace W, ZopfliArgs Z, int ph
   if (phase == 1) {
     const uint32_t mb_span = P.unit * P.mb_units, mb_lo = s / mb_span * mb_span, mb_hi = bmin(P.n, mb_lo + mb_span);
     warm_dc[0] = warm_dc[1] = warm_dc[2] = warm_dc[3] = 0x3fffffff;
-    if (P.hq_warm && (u % P.mb_units) != 0 && s >= HQ_WARMUP_BYTES) {  // incoming distance cache (bro_hq.cuh:hq_warm_start_cache)
+    if ((u % P.mb_units) != 0 && s >= HQ_WARMUP_BYTES) {  // incoming distance cache (bro_hq.cuh:hq_warm_start_cache)
       const int32_t unknown[4] = {0x3fffffff, 0x3fffffff, 0x3fffffff, 0x3fffffff};
       HqUnit V = U;
       V.ustart = s - HQ_WARMUP_BYTES; V.len = HQ_WARMUP_BYTES; V.start_dc = unknown;

@@ -21,6 +21,13 @@ BRO_HD uint32_t chunk_len_at(uint64_t done, uint64_t total) {
   return (uint32_t)(left < BRO_CHUNK_BYTES ? left : BRO_CHUNK_BYTES);
 }
 
+// The quality the encoder runs for a requested one: 5..9 hash-chain family (encode.rs:834-893), 10 / 11 shortest-path parse;
+// q0..q4 (BasicHasher H2..H54, fragment compressors) are not built and run as 5.
+BRO_HD int effective_quality(int requested_quality) {
+  return requested_quality < 5 ? 5 : (requested_quality > 11 ? 11 : requested_quality);
+}
+
+// The defaults of every configuration are set by default_enc_params() (bro_hq.cuh), which the encoder and its CPU model share.
 struct EncParams {
   int quality;        // 5..11
   int lgwin;          // 10..24
@@ -36,13 +43,10 @@ struct EncParams {
   uint32_t n;         // size of the range being compressed (positions are relative to its start)
   uint32_t abs_base;  // absolute stream position of relative position 0 (window limit at the stream start)
   uint32_t size_hint;
-  int use_rle_opt;    // apply BrotliOptimizeHuffmanCountsForRle
-  int split;          // greedy block splitting on/off
   int ctx_model;      // literal context modelling on/off
   int use_dict;       // static-dictionary matches on/off
   int hq_split;       // quality >= 10: 1 = BrotliSplitBlock + clustered context maps (default), 0 = the greedy splitter of q5..q9
   int hq_levels;      // quality >= 10: number of long-prefix candidate levels (8, 16, 32 bytes) on top of the 4-byte buckets: 0..3
-  int hq_warm;        // quality >= 10: parse units learn their incoming distance cache from the HQ_WARMUP_BYTES in front of them
 };
 
 // ---- scores ----

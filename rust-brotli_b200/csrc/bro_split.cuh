@@ -170,7 +170,7 @@ struct SplitResult {
 
 // symbols: for nctx == 1 the symbol itself; otherwise literal | ctx << 8
 inline void greedy_split(const uint16_t* syms, uint32_t count, uint32_t A, uint32_t nctx, uint32_t min_block,
-                         uint32_t thr_bits, bool enable, const uint32_t* lut, SplitResult* out) {
+                         uint32_t thr_bits, const uint32_t* lut, SplitResult* out) {
   const uint32_t HA = nctx * A;
   const uint32_t max_types = nctx == 1 ? 256u : 256u / nctx;
   std::vector<uint32_t> hist((size_t)(max_types + 1) * HA, 0);  // slot t = block type t, slot num_types = pending
@@ -231,22 +231,12 @@ inline void greedy_split(const uint16_t* syms, uint32_t count, uint32_t A, uint3
     }
     pending = 0;
   };
-  if (!enable) {
-    for (uint32_t i = 0; i < count; ++i) {
-      uint32_t sym = nctx == 1 ? syms[i] : (syms[i] & 0xFF) + (syms[i] >> 8) * A;
-      ++hist[sym];
-    }
-    out->types.push_back(0);
-    out->lengths.push_back(count < min_block ? min_block : count);
-    s.num_types = 1;
-  } else {
-    for (uint32_t i = 0; i < count; ++i) {
-      uint32_t sym = nctx == 1 ? syms[i] : (syms[i] & 0xFF) + (syms[i] >> 8) * A;
-      ++hist[(size_t)s.num_types * HA + sym];
-      if (++pending == s.target_block_size) finish(false);
-    }
-    finish(true);
+  for (uint32_t i = 0; i < count; ++i) {
+    uint32_t sym = nctx == 1 ? syms[i] : (syms[i] & 0xFF) + (syms[i] >> 8) * A;
+    ++hist[(size_t)s.num_types * HA + sym];
+    if (++pending == s.target_block_size) finish(false);
   }
+  finish(true);
   out->num_types = s.num_types;
   out->histograms.assign(hist.begin(), hist.begin() + (size_t)s.num_types * HA);
   out->starts.resize(out->lengths.size());

@@ -72,7 +72,7 @@ def test_model_edge_sizes(model, n):
 def test_model_options(model):
     d = golden_bytes("asyoulik.txt")
     base, _ = model.compress(d, 5, 22)
-    for kw in ({"split": 0}, {"ctx_model": 0}, {"use_rle_opt": 0}, {"unit": 2048}, {"unit": 16384}, {"lcap": 32}, {"mb_units": 8}):
+    for kw in ({"ctx_model": 0}, {"unit": 2048}, {"unit": 16384}, {"lcap": 32}, {"mb_units": 8}):
         c, _ = model.compress(d, 5, 22, **kw)
         assert sys_decompress(c, len(d)) == d
         assert len(c) < len(base) * 1.03

@@ -6,7 +6,7 @@ _ROOT = os.path.dirname(_HERE)
 class EncParams(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int) for n in ("quality", "lgwin", "hash_type", "key_bits", "hash_len", "depth", "n_last")] + \
                [(n, ctypes.c_uint32) for n in ("lcap", "unit", "mb_units", "max_backward", "n", "abs_base", "size_hint")] + \
-               [(n, ctypes.c_int) for n in ("use_rle_opt", "split", "ctx_model", "use_dict", "hq_split", "hq_levels", "hq_warm")]
+               [(n, ctypes.c_int) for n in ("ctx_model", "use_dict", "hq_split", "hq_levels")]
 
 class ModelStats(ctypes.Structure):
     _fields_ = [(n, ctypes.c_uint64) for n in ("num_metablocks", "num_raw_metablocks", "num_commands", "num_literals", "header_bits", "body_bits")] + \
