@@ -148,12 +148,44 @@ uint32_t b200_last_multi_device_mask(void);
 int b200_encoder_set_option(B200Encoder* e, int option, uint32_t value);
 size_t b200_max_compressed_size(size_t n);
 /* device_io: 0 = in / out are host pointers; 1 = both are device pointers on the encoder's GPU; 2 = host input, device output
- * (e.g. shard outputs that travel on to a peer GPU over NVLink); 3 = device input, host output */
+ * (e.g. shard outputs that travel on to a peer GPU over NVLink); 3 = device input, host output.
+ * These calls return when the output is in place.  They run on the encoder's own streams, which do not wait for any other
+ * stream: device input written by a kernel on another stream (a torch stream, the legacy default stream) must be complete
+ * before the call, e.g. after torch.cuda.synchronize().  b200_encoder_compress_range_async has no such hazard. */
 int b200_encoder_compress(B200Encoder* e, int quality, int lgwin, const uint8_t* in, size_t n, uint8_t* out, size_t out_cap,
                           size_t* out_size, int device_io);
 int b200_encoder_compress_range(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n,
                                 size_t range_start, size_t range_len, int first, int last, int byte_align, uint8_t* out,
                                 size_t out_cap, size_t* out_size, int device_io);
+/* Sizes every device buffer, per-lane workspace and event that a call with these arguments uses. After this call, an async
+ * call with the same or smaller (quality, lgwin, size_hint, n, range_len) allocates nothing, as long as the encoder's options
+ * (number of lanes, quality 10 / 11 parse unit and splitter) stay the same.  size_hint 0 = n.  Returns 0 if memory runs out. */
+int b200_encoder_reserve(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, size_t n, size_t range_len);
+/* b200_encoder_compress_range, stream-ordered.  in / out / out_size are device pointers on the encoder's GPU; stream is a
+ * cudaStream_t passed as void* (0 = the legacy default stream).  Returns 1 when the work has been enqueued.  out[0, *out_size)
+ * is the compressed range once `stream` reaches that point; nothing on the host waits for it.  The bytes equal those of
+ * b200_encoder_compress_range with the same arguments.
+ *  - Ordering: the input is read only after the work enqueued on `stream` before the call; the output and *out_size are
+ *    written before any work enqueued on `stream` after the call.  The call forks from `stream` into the encoder's streams with
+ *    one event and joins back with a wait on the last event of each encoder stream it used.
+ *  - Calls on one encoder run one at a time on the device: outside a graph capture, each async or blocking call first waits,
+ *    on the device, for the encoder's previous call.
+ *  - Output: the stream is built directly in `out`, which the call zeroes first; no staging buffer and no copy.  Refused (0,
+ *    nothing enqueued): out_cap < b200_max_compressed_size(range_len) + 64, `out` not 4-byte aligned, in / out / out_size not
+ *    device memory of the encoder's GPU, n >= 0xFFFFF000, a range outside [0, n).  `in` is not read when range_len == 0.
+ *  - Empty input (n == 0 or range_len == 0: the single byte 6 of an empty stream when first && last && n == 0, otherwise
+ *    nothing) is enqueued like any other call.
+ *  - Allocation: a call whose buffers are too small grows them, and cudaFree may then block the host until the device is
+ *    idle.  b200_encoder_reserve beforehand avoids that.
+ *  - CUDA graph capture (`stream` capturing): the call never allocates, creates no event and does not wait for work recorded
+ *    outside the capture.  If a buffer would have to grow it returns 0 before it enqueues anything, so the capture stays
+ *    valid: reserve first.  Once a call has been captured the encoder's workspace is frozen, since the graph points into it:
+ *    any later call (async or blocking) that would grow it is refused.  A graph replay does not order itself after other
+ *    calls on the encoder, nor they after it: do not use an encoder captured in a graph while a replay may be in flight.
+ *  - Stage timing (B200_OPT_TIMING) is not collected for these calls. */
+int b200_encoder_compress_range_async(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n,
+                                      size_t range_start, size_t range_len, int first, int last, int byte_align, uint8_t* out,
+                                      size_t out_cap, uint64_t* out_size, void* stream);
 int b200_encoder_last_timings(B200Encoder* e, float* ms, uint32_t* launches);
 /* stage hook of quality 5..9: best[] of the match stage (distance << 8 | capped length, or a static-dictionary candidate) for
  * [range_start, range_start + range_len) of an n-byte buffer, range_len <= one chunk; size_hint 0 = n.  search = 0: the up-front

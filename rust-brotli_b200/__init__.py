@@ -129,6 +129,36 @@ def encoder_compress(data: bytes, quality: int = 11, lgwin: int = 22) -> bytes:
     return out.raw[:osz.value]
 
 
+_tensor_encoders = {}  # CUDA ordinal -> the DeviceEncoder compress_tensor uses when it is given none
+
+
+def compress_tensor(t, quality: int = 5, lgwin: int = 22, encoder: DeviceEncoder = None):
+    """Compresses a contiguous uint8 CUDA tensor on ``torch.cuda.current_stream()`` without waiting for it.
+
+    Returns ``(out, size)``: a uint8 tensor of capacity bytes whose first ``size`` bytes become the brotli stream, and a
+    one-element int64 tensor holding that size, both on ``t``'s device and both written in the order of the current stream (read
+    them after it, e.g. ``out[:size.item()]``, which synchronises).  Nothing here synchronises.  Inside ``torch.cuda.graph``
+    pass an ``encoder`` on which ``reserve(quality, lgwin, t.numel())`` was called before the capture.
+    """
+    import torch
+    if not (t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
+        raise ValueError("compress_tensor needs a contiguous uint8 CUDA tensor")
+    dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
+    if encoder is None:
+        encoder = _tensor_encoders.get(dev)
+        if encoder is None:
+            encoder = _tensor_encoders[dev] = DeviceEncoder(dev)
+    elif encoder.device != dev:
+        raise ValueError("the encoder is on cuda:%d, the tensor on cuda:%d" % (encoder.device, dev))
+    n = t.numel()
+    cap = lib().b200_max_compressed_size(n) + 64
+    out = torch.empty(cap, dtype=torch.uint8, device=t.device)
+    size = torch.empty(1, dtype=torch.int64, device=t.device)
+    stream = torch.cuda.current_stream(t.device)
+    encoder.compress_async(t.data_ptr(), n, out.data_ptr(), cap, size.data_ptr(), quality, lgwin, stream.cuda_stream)
+    return out, size
+
+
 class _Stream:
     """BrotliEncoderState driven through BrotliEncoderCompressStream, as writer.rs / reader.rs do."""
 

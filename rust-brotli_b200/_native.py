@@ -37,6 +37,11 @@ def lib():
         L.b200_encoder_compress_range.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.c_uint64, vp, sz, sz, sz, ctypes.c_int,
                                                   ctypes.c_int, ctypes.c_int, vp, sz, ctypes.POINTER(sz), ctypes.c_int]
         L.b200_encoder_compress_range.restype = ctypes.c_int
+        L.b200_encoder_reserve.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.c_uint64, sz, sz]
+        L.b200_encoder_reserve.restype = ctypes.c_int
+        L.b200_encoder_compress_range_async.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.c_uint64, vp, sz, sz, sz, ctypes.c_int,
+                                                        ctypes.c_int, ctypes.c_int, vp, sz, vp, vp]
+        L.b200_encoder_compress_range_async.restype = ctypes.c_int
         L.b200_encoder_last_timings.argtypes = [vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_uint32)]
         L.b200_stage_match.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.c_uint64, vp, sz, sz, sz, ctypes.c_int, vp]
         L.b200_stage_match.restype = ctypes.c_int
@@ -110,6 +115,28 @@ class DeviceEncoder:
         if not ok:
             raise RuntimeError("b200_encoder_compress (device io) failed")
         return osz.value
+
+    def reserve(self, quality: int, lgwin: int, n: int, range_len=None, size_hint: int = 0):
+        """Allocates everything an async call of these or smaller arguments uses (b200_encoder_reserve): such calls then never
+        allocate, which a call inside a CUDA graph capture requires."""
+        if not self._L.b200_encoder_reserve(self._h, quality, lgwin, size_hint, n, n if range_len is None else range_len):
+            raise RuntimeError("b200_encoder_reserve failed")
+
+    def compress_async(self, d_in_ptr: int, n: int, d_out_ptr: int, out_cap: int, d_size_ptr: int, quality: int, lgwin: int,
+                       stream_ptr: int, range_start: int = 0, range_len=None, first: bool = True, last: bool = True,
+                       byte_align: bool = False, size_hint: int = 0):
+        """Enqueues the compression of [range_start, range_start + range_len) of the n device bytes at d_in_ptr on the CUDA stream
+        stream_ptr (e.g. torch.cuda.current_stream().cuda_stream) and returns without waiting: out[0, size) and the uint64 size at
+        d_size_ptr are written when the stream gets there (b200_encoder_compress_range_async).  Raises if the call is refused;
+        nothing is enqueued then."""
+        if range_len is None:
+            range_len = n - range_start
+        ok = self._L.b200_encoder_compress_range_async(self._h, quality, lgwin, size_hint, ctypes.c_void_p(d_in_ptr), n, range_start,
+                                                        range_len, int(first), int(last), int(byte_align),
+                                                        ctypes.c_void_p(d_out_ptr), out_cap, ctypes.c_void_p(d_size_ptr),
+                                                        ctypes.c_void_p(stream_ptr))
+        if not ok:
+            raise RuntimeError("b200_encoder_compress_range_async refused the call")
 
     def timings(self):
         ms = (ctypes.c_float * NUM_STAGES)()

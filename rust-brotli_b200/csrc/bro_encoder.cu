@@ -35,8 +35,13 @@ namespace {
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
+  bool frozen = false;  // a captured CUDA graph points into the buffer: it may not be freed or moved
   bool ensure(size_t bytes) {
     if (bytes <= cap) return true;
+    if (frozen) {
+      fprintf(stderr, "[brotli_b200] workspace frozen by a CUDA graph capture cannot grow to %zu bytes\n", bytes);
+      return false;
+    }
     if (p) cudaFree(p);
     p = nullptr;
     cap = 0;
@@ -73,6 +78,13 @@ struct EventPool {
       ev.push_back(e);
     }
     return ev[used++];
+  }
+  void reserve(size_t n) {  // untimed events, so that a call inside a graph capture creates none
+    while (ev.size() < n) {
+      cudaEvent_t e;
+      if (cudaEventCreateWithFlags(&e, cudaEventDisableTiming) != cudaSuccess) return;
+      ev.push_back(e);
+    }
   }
   void reset() { used = 0; }
   void destroy() { for (auto& e : ev) cudaEventDestroy(e); ev.clear(); used = 0; }
@@ -258,6 +270,46 @@ void layout_chunk(Carve& a, uint32_t c, const EncParams& P, Workspace* W, ChunkB
   }
 }
 
+// bytes of lane arena a chunk of c bytes uses (the sizing pass of run_chunk)
+size_t chunk_arena_bytes(const EncParams& P, uint32_t c) {
+  Workspace W;
+  ChunkBufs X;
+  memset(&W, 0, sizeof(W));
+  memset(&X, 0, sizeof(X));
+  Carve sizing{nullptr};
+  layout_chunk(sizing, c, P, &W, &X);
+  return sizing.off;
+}
+
+// What one call compresses: its parameters, the span of the input that is staged on the device (the range and the window in
+// front of it) and the range's chunks.
+struct CallPlan {
+  EncParams P;
+  size_t base = 0, end = 0, staged = 0;  // absolute positions: staged = end - base bytes from base on
+  size_t need = 0;                       // output bytes the chunks may touch (zeroed before they run)
+  std::vector<std::pair<size_t, size_t>> chunks;  // (absolute start, length)
+};
+
+// The device memory and events a call uses, apart from the blocking path's d_out and pinned totals.
+struct CallSizes {
+  size_t data = 0, total = 0, events = 0, arena[kMaxLanes] = {};
+  void cover(const CallSizes& o) {
+    data = std::max(data, o.data);
+    total = std::max(total, o.total);
+    events = std::max(events, o.events);
+    for (int i = 0; i < kMaxLanes; ++i) arena[i] = std::max(arena[i], o.arena[i]);
+  }
+};
+
+bool on_device(const void* p, int device) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();
+    return false;
+  }
+  return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == device;
+}
+
 }  // namespace
 
 struct B200Encoder {
@@ -277,6 +329,7 @@ struct B200Encoder {
   uint64_t* h_total = nullptr;                   // pinned mirror of d_total[1 + k]
   size_t h_total_cap = 0;
   EventPool sync_events;
+  cudaEvent_t ev_call = nullptr;  // end of the last stream-ordered call outside a capture: the next call starts behind it
   uint64_t data_base = 0;  // absolute stream position of d_data[0]
   float stage_ms[B200_NUM_STAGES];
   uint32_t launches = 0;
@@ -291,6 +344,7 @@ struct B200Encoder {
     for (auto& L : lanes) CUDA_OK(cudaStreamCreateWithFlags(&L.stream, cudaStreamNonBlocking));
     CUDA_OK(cudaStreamCreateWithFlags(&s_in, cudaStreamNonBlocking));
     CUDA_OK(cudaStreamCreateWithFlags(&s_out, cudaStreamNonBlocking));
+    CUDA_OK(cudaEventCreateWithFlags(&ev_call, cudaEventDisableTiming));
     if (!d_lut.ensure(65536 * 4)) return false;
     std::vector<uint32_t> lut(65536);
     fill_log2_q16_lut(lut.data());
@@ -320,6 +374,7 @@ struct B200Encoder {
     for (auto* b : all) b->release();
     if (h_total) cudaFreeHost(h_total);
     sync_events.destroy();
+    if (ev_call) cudaEventDestroy(ev_call);
     if (s_in) cudaStreamDestroy(s_in);
     if (s_out) cudaStreamDestroy(s_out);
   }
@@ -347,6 +402,55 @@ struct B200Encoder {
         P->mb_units = span / P->unit;
       }
     }
+  }
+
+  void plan_call(CallPlan* c, int quality, int lgwin, uint64_t size_hint, size_t range_start, size_t range_len) const {
+    fill_params(&c->P, quality, lgwin, size_hint);
+    const size_t window = (size_t)1 << c->P.lgwin;
+    c->base = range_start > window ? ((range_start - window) & ~(size_t)4095) : 0;
+    c->end = range_start + range_len;
+    c->staged = c->end - c->base;
+    c->need = b200_max_compressed_size(range_len) + 64;
+    c->chunks.clear();
+    for (size_t done = 0; done < range_len;) {
+      const size_t len = chunk_len_at(done, range_len);
+      c->chunks.emplace_back(range_start + done, len);
+      done += len;
+    }
+  }
+  // chunk k runs on lane k % num_lanes; a call without chunks uses nothing
+  CallSizes sizes_of(const CallPlan& c) const {
+    CallSizes s;
+    const size_t nchunks = c.chunks.size();
+    if (!nchunks) return s;
+    s.data = c.staged + kPad;
+    s.total = (nchunks + 2) * 8;
+    s.events = 3 * nchunks + kMaxLanes + 2;  // blocking: in / layout / done per chunk; async: in / layout per chunk, fork, joins
+    for (size_t k = 0; k < nchunks; ++k) {
+      size_t& a = s.arena[k % (size_t)num_lanes];
+      a = std::max(a, chunk_arena_bytes(c.P, (uint32_t)c.chunks[k].second));
+    }
+    return s;
+  }
+  // Puts the buffers and events of s in place (grow), or only checks that they are (a call inside a graph capture may not
+  // allocate).  Growing frees the old buffer, and cudaFree waits for the device.
+  bool provide(const CallSizes& s, bool grow) {
+    if (!grow) {
+      if (d_data.cap < s.data || d_total.cap < s.total || sync_events.ev.size() < s.events) return false;
+      for (int i = 0; i < kMaxLanes; ++i)
+        if (lanes[i].arena.cap < s.arena[i]) return false;
+      return true;
+    }
+    if (!d_data.ensure(s.data) || !d_total.ensure(s.total)) return false;
+    for (int i = 0; i < kMaxLanes; ++i)
+      if (!lanes[i].arena.ensure(s.arena[i])) return false;
+    sync_events.reserve(s.events);
+    return sync_events.ev.size() >= s.events;
+  }
+  // a captured graph holds pointers into these buffers from now on
+  void freeze() {
+    d_data.frozen = d_total.frozen = true;
+    for (auto& L : lanes) L.arena.frozen = true;
   }
 
   // Enqueues on `stream` the stable sort of the batch positions 0..count-1 (input bytes at `data`, 4096-byte aligned and padded)
@@ -658,51 +762,27 @@ int b200_encoder_set_option(B200Encoder* e, int option, uint32_t value) {
 
 size_t b200_max_compressed_size(size_t n) { return n + (n >> 10) * 8 + 4096; }
 
-// Compresses [range_start, range_start+range_len) of an n-byte stream.  in/out are device pointers when
-// device_io != 0, host pointers otherwise.  first/last: emit stream header / final empty metablock;
-// byte_align: end the range with a padding metablock so that ranges can be concatenated with memcpy.
+// Stages the input of plan c on s_in and enqueues its chunks on the lanes; their metablocks are written into `out` (c.need
+// bytes, zeroed here first).  The caller has made s_in wait for whatever the call is ordered after.  h_done (blocking path):
+// each chunk's end bit position is copied to h_total[k] on its lane and h_done[k] is recorded behind it.
 //
-// Pipeline: the input is staged chunk by chunk on a copy stream, chunks alternate between two compute lanes, and the
-// finished part of the output is copied back while later chunks are still running.
-static bool compress_range_impl(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n,
-                                size_t range_start, size_t range_len, bool first, bool last, bool byte_align, uint8_t* out,
-                                size_t out_cap, size_t* out_size, int device_io, bool keep_on_device) {
-  e->launches = 0;
-  e->reset_timings();
-  e->sync_events.reset();
-  EncParams P;
-  e->fill_params(&P, quality, lgwin, size_hint ? size_hint : n);
-  const size_t window = (size_t)1 << P.lgwin;
-  const size_t base = range_start > window ? ((range_start - window) & ~(size_t)4095) : 0;
-  const size_t end = range_start + range_len;
-  const size_t staged = end - base;
-  const size_t need = b200_max_compressed_size(range_len) + 64;
-  std::vector<std::pair<size_t, size_t>> chunks;  // (absolute start, length)
-  for (size_t done = 0; done < range_len;) {
-    const size_t len = chunk_len_at(done, range_len);
-    chunks.emplace_back(range_start + done, len);
-    done += len;
-  }
-  const size_t nchunks = chunks.size();
-  // device_io: 0 host in / host out, 1 device in / device out, 2 host in / device out, 3 device in / host out
-  const bool in_dev = device_io == 1 || device_io == 3, out_dev = device_io == 1 || device_io == 2;
-  const cudaMemcpyKind in_kind = in_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-  const cudaMemcpyKind out_kind = out_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-  if (!e->d_data.ensure(staged + kPad) || !e->d_out.ensure(need) || !e->ensure_totals(nchunks)) return false;
-  e->data_base = base;
+// Pipeline: the input is staged chunk by chunk on a copy stream and chunks alternate between the compute lanes.
+static bool enqueue_range(B200Encoder* e, const CallPlan& c, const uint8_t* in, cudaMemcpyKind in_kind, uint8_t* out, bool first,
+                          bool last, bool byte_align, std::vector<cudaEvent_t>* h_done) {
+  const size_t nchunks = c.chunks.size();
+  e->data_base = c.base;
   uint8_t* dd = e->d_data.as<uint8_t>();
-  CUDA_OK(cudaMemsetAsync(e->d_out.p, 0, need, e->s_in));
+  CUDA_OK(cudaMemsetAsync(out, 0, c.need, e->s_in));
   CUDA_OK(cudaMemsetAsync(e->d_total.p, 0, 8, e->s_in));
-  CUDA_OK(cudaMemsetAsync(dd + staged, 0, kPad, e->s_in));
-  std::vector<cudaEvent_t> ev_done(nchunks);
+  CUDA_OK(cudaMemsetAsync(dd + c.staged, 0, kPad, e->s_in));
   cudaEvent_t prev_layout = nullptr;
-  size_t copied = base;  // absolute position up to which the input is staged
+  size_t copied = c.base;  // absolute position up to which the input is staged
   for (size_t k = 0; k < nchunks; ++k) {
-    const size_t s = chunks[k].first, len = chunks[k].second;
+    const size_t s = c.chunks[k].first, len = c.chunks[k].second;
     // stage the input this chunk can see: its window halo (first chunk), its own bytes, a short look-ahead
-    const size_t upto = std::min(end, s + len + kLookahead);
+    const size_t upto = std::min(c.end, s + len + kLookahead);
     if (upto > copied) {
-      CUDA_OK(cudaMemcpyAsync(dd + (copied - base), in + copied, upto - copied, in_kind, e->s_in));
+      CUDA_OK(cudaMemcpyAsync(dd + (copied - c.base), in + copied, upto - copied, in_kind, e->s_in));
       copied = upto;
     }
     cudaEvent_t ev_in = e->sync_events.get(false);
@@ -711,14 +791,43 @@ static bool compress_range_impl(B200Encoder* e, int quality, int lgwin, uint64_t
     CUDA_OK(cudaStreamWaitEvent(L.stream, ev_in, 0));
     cudaEvent_t ev_layout = e->sync_events.get(false);
     const bool f = first && k == 0, l = k + 1 == nchunks;
-    if (!e->run_chunk(L, P, (uint32_t)s, (uint32_t)len, e->d_out.as<uint32_t>(), need, f, last && l, byte_align && l, (uint32_t)k,
-                      prev_layout, ev_layout))
+    if (!e->run_chunk(L, c.P, (uint32_t)s, (uint32_t)len, reinterpret_cast<uint32_t*>(out), c.need, f, last && l, byte_align && l,
+                      (uint32_t)k, prev_layout, ev_layout))
       return false;
     prev_layout = ev_layout;
-    CUDA_OK(cudaMemcpyAsync(e->h_total + k, e->d_total.as<uint64_t>() + 1 + k, 8, cudaMemcpyDeviceToHost, L.stream));
-    ev_done[k] = e->sync_events.get(false);
-    CUDA_OK(cudaEventRecord(ev_done[k], L.stream));
+    if (h_done) {
+      CUDA_OK(cudaMemcpyAsync(e->h_total + k, e->d_total.as<uint64_t>() + 1 + k, 8, cudaMemcpyDeviceToHost, L.stream));
+      (*h_done)[k] = e->sync_events.get(false);
+      CUDA_OK(cudaEventRecord((*h_done)[k], L.stream));
+    }
   }
+  return true;
+}
+
+// Compresses [range_start, range_start+range_len) of an n-byte stream and returns when the output is in place.  in/out are
+// device pointers when device_io != 0, host pointers otherwise.  first/last: emit stream header / final empty metablock;
+// byte_align: end the range with a padding metablock so that ranges can be concatenated with memcpy.
+//
+// The stream is built in d_out; as each chunk finishes, the finished part of the output is copied to `out` while later chunks
+// are still running.
+static bool compress_range_impl(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n,
+                                size_t range_start, size_t range_len, bool first, bool last, bool byte_align, uint8_t* out,
+                                size_t out_cap, size_t* out_size, int device_io, bool keep_on_device) {
+  e->launches = 0;
+  e->reset_timings();
+  e->sync_events.reset();
+  CallPlan c;
+  e->plan_call(&c, quality, lgwin, size_hint ? size_hint : n, range_start, range_len);
+  const size_t nchunks = c.chunks.size();
+  // device_io: 0 host in / host out, 1 device in / device out, 2 host in / device out, 3 device in / host out
+  const bool in_dev = device_io == 1 || device_io == 3, out_dev = device_io == 1 || device_io == 2;
+  const cudaMemcpyKind in_kind = in_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+  const cudaMemcpyKind out_kind = out_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  // the whole workspace is in place before the first launch: growing a buffer (cudaFree) waits for the device
+  if (!e->provide(e->sizes_of(c), true) || !e->d_out.ensure(c.need) || !e->ensure_totals(nchunks)) return false;
+  CUDA_OK(cudaStreamWaitEvent(e->s_in, e->ev_call, 0));  // behind the encoder's last stream-ordered call
+  std::vector<cudaEvent_t> ev_done(nchunks);
+  if (!enqueue_range(e, c, in, in_kind, e->d_out.as<uint8_t>(), first, last, byte_align, &ev_done)) return false;
   // drain: as each chunk finishes, every output byte below its end bit position is final
   size_t done_bytes = 0;
   for (size_t k = 0; k < nchunks; ++k) {
@@ -738,6 +847,108 @@ static bool compress_range_impl(B200Encoder* e, int quality, int lgwin, uint64_t
   *out_size = done_bytes;
   if (e->timing) e->collect_timings();
   return true;
+}
+
+// The stream-ordered ending (b200_encoder_compress_range_async): the call forks from `st` into s_in (and through s_in's events
+// into the lanes), joins back into `st` behind the last work of s_in and of every lane it used, and writes *out_size with one
+// more launch on `st`.  Inside a capture it neither waits for nor records ev_call: a graph may not depend on work outside it.
+static bool enqueue_async(B200Encoder* e, const CallPlan& c, const uint8_t* in, bool first, bool last, bool byte_align,
+                          bool empty_stream, uint8_t* out, uint64_t* out_size, cudaStream_t st, bool capturing) {
+  const size_t nchunks = c.chunks.size();
+  cudaEvent_t fork = e->sync_events.get(false);
+  CUDA_OK(cudaEventRecord(fork, st));
+  CUDA_OK(cudaStreamWaitEvent(e->s_in, fork, 0));
+  if (!capturing) CUDA_OK(cudaStreamWaitEvent(e->s_in, e->ev_call, 0));
+  if (nchunks) {
+    if (!enqueue_range(e, c, in, cudaMemcpyDeviceToDevice, out, first, last, byte_align, nullptr)) return false;
+  } else {
+    CUDA_OK(cudaMemsetAsync(out, 0, c.need, e->s_in));
+  }
+  cudaStream_t used[kMaxLanes + 1];
+  size_t nused = 0;
+  used[nused++] = e->s_in;
+  for (size_t i = 0; i < std::min(nchunks, (size_t)e->num_lanes); ++i) used[nused++] = e->lanes[i].stream;
+  for (size_t i = 0; i < nused; ++i) {
+    cudaEvent_t join = e->sync_events.get(false);
+    CUDA_OK(cudaEventRecord(join, used[i]));
+    CUDA_OK(cudaStreamWaitEvent(st, join, 0));
+  }
+  k_out_size<<<1, 1, 0, st>>>(nchunks ? e->d_total.as<uint64_t>() + nchunks : nullptr, out, empty_stream ? 1 : 0, out_size);
+  e->launches += 1;
+  CUDA_OK(cudaGetLastError());
+  if (!capturing) CUDA_OK(cudaEventRecord(e->ev_call, st));
+  return true;
+}
+
+int b200_encoder_reserve(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, size_t n, size_t range_len) {
+  if (!e || !e->ok || n >= 0xFFFFF000ull || range_len > n) return 0;
+  if (cudaSetDevice(e->device) != cudaSuccess) return 0;
+  // Every call with the same or smaller arguments must fit.  Workspaces grow with the range and the window, but not with the
+  // quality or the size hint: smaller parse units (quality 10 against 11, small size hints at 10 / 11) need more per byte.  So
+  // each quality family up to `quality` is sized at each size-hint class up to `size_hint`; the staged input is bounded over
+  // every range start.
+  const uint64_t hint = size_hint ? size_hint : n;
+  const int q_max = effective_quality(quality);
+  const uint64_t hints[3] = {hint, std::min<uint64_t>(hint, 1u << 20), std::min<uint64_t>(hint, 256u << 10)};
+  CallSizes s;
+  for (int q : {5, 10, 11}) {
+    if (q > q_max) break;
+    for (uint64_t h : hints) {
+      if (!h) continue;
+      CallPlan c;
+      e->plan_call(&c, q, lgwin, h, n - range_len, range_len);
+      s.cover(e->sizes_of(c));
+    }
+  }
+  if (range_len) {
+    EncParams P;
+    e->fill_params(&P, quality, lgwin, hint);
+    s.data = std::min<size_t>(n, range_len + ((size_t)1 << P.lgwin) + 4095) + kPad;
+  }
+  return e->provide(s, true) ? 1 : 0;
+}
+
+int b200_encoder_compress_range_async(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n,
+                                      size_t range_start, size_t range_len, int first, int last, int byte_align, uint8_t* out,
+                                      size_t out_cap, uint64_t* out_size, void* stream) {
+  if (!e || !e->ok || !out || !out_size) return 0;
+  if (n >= 0xFFFFF000ull || range_start > n || range_len > n - range_start) return 0;  // 32-bit positions
+  if (cudaSetDevice(e->device) != cudaSuccess) return 0;
+  if (out_cap < b200_max_compressed_size(range_len) + 64 || (reinterpret_cast<uintptr_t>(out) & 3)) return 0;
+  // (the pointer queries run in relaxed capture mode: under a global-mode capture on another stream they are no reason to fail)
+  cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+  if (cudaThreadExchangeStreamCaptureMode(&mode) != cudaSuccess) return 0;
+  const bool placed = on_device(out, e->device) && on_device(out_size, e->device) && (!range_len || on_device(in, e->device));
+  cudaThreadExchangeStreamCaptureMode(&mode);
+  if (!placed) return 0;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaStreamCaptureStatus cs;
+  if (cudaStreamIsCapturing(st, &cs) != cudaSuccess) {
+    cudaGetLastError();
+    return 0;
+  }
+  if (cs == cudaStreamCaptureStatusInvalidated) return 0;
+  const bool capturing = cs == cudaStreamCaptureStatusActive;
+  CallPlan c;
+  e->plan_call(&c, quality, lgwin, size_hint ? size_hint : n, range_start, range_len);
+  if (!e->provide(e->sizes_of(c), !capturing)) {
+    if (capturing) fprintf(stderr, "[brotli_b200] a call inside a CUDA graph capture needs b200_encoder_reserve first\n");
+    return 0;
+  }
+  if (capturing) e->freeze();
+  e->launches = 0;
+  e->reset_timings();
+  e->sync_events.reset();
+  const bool timing = e->timing;
+  e->timing = false;  // stage timing would read events back on the host
+  const bool ok = enqueue_async(e, c, in, first != 0, last != 0, byte_align != 0, first && last && n == 0, out, out_size, st,
+                                capturing);
+  e->timing = timing;
+  if (!ok) {
+    if (!capturing) cudaDeviceSynchronize();  // leave no work in flight behind a failed call
+    return 0;
+  }
+  return 1;
 }
 
 int b200_encoder_compress_range(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n,
@@ -846,7 +1057,8 @@ int b200_stage_sort(B200Encoder* e, int quality, int lgwin, const uint8_t* in, s
   const SortBufs S = layout_sort(carve, (uint32_t)n);
   e->data_base = 0;
   uint8_t* dd = e->d_data.as<uint8_t>();
-  bool ok = cudaMemcpyAsync(dd, in, n, cudaMemcpyHostToDevice, L.stream) == cudaSuccess &&
+  bool ok = cudaStreamWaitEvent(L.stream, e->ev_call, 0) == cudaSuccess &&
+            cudaMemcpyAsync(dd, in, n, cudaMemcpyHostToDevice, L.stream) == cudaSuccess &&
             cudaMemsetAsync(dd + n, 0, kPad, L.stream) == cudaSuccess;
   if (!ok) return 0;
   if (level < 0) e->run_sort<false>(L.stream, S, dd, (uint32_t)n, P.hash_type, P.key_bits);

@@ -21,6 +21,10 @@ int b200_encoder_compress(B200Encoder* e, int quality, int lgwin, const uint8_t*
 int b200_encoder_compress_range(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n,
                                 size_t range_start, size_t range_len, int first, int last, int byte_align, uint8_t* out,
                                 size_t out_cap, size_t* out_size, int device_io);
+int b200_encoder_reserve(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, size_t n, size_t range_len);
+int b200_encoder_compress_range_async(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n,
+                                      size_t range_start, size_t range_len, int first, int last, int byte_align, uint8_t* out,
+                                      size_t out_cap, uint64_t* out_size, void* stream);
 int b200_encoder_last_timings(B200Encoder* e, float* ms /* [B200_NUM_STAGES] */, uint32_t* launches);
 int b200_stage_match(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n, size_t range_start,
                      size_t range_len, int search, uint32_t* best_out);

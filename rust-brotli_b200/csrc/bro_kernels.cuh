@@ -2273,6 +2273,18 @@ __global__ void k_layout(Workspace W, int first, int last, int byte_align, uint6
   *total_after = pos;  // per-chunk copy: the host reads it while later chunks keep advancing total_bits
 }
 
+// Single thread, last launch of a stream-ordered call: the byte size of the range's output, from the end bit position of its last
+// chunk (end_bits), or -- a call without chunks -- of the empty stream (encode.rs:1463-1467: one byte 6) or of nothing.
+__global__ void k_out_size(const uint64_t* end_bits, uint8_t* out, int empty_stream, uint64_t* out_size) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  if (end_bits) {
+    *out_size = (*end_bits + 7) >> 3;
+    return;
+  }
+  if (empty_stream) out[0] = 6;
+  *out_size = empty_stream ? 1 : 0;
+}
+
 __global__ void __launch_bounds__(256) k_emit_header(Workspace W) {
   const uint32_t m = blockIdx.x;
   const MBDesc& mb = W.mb[m];

@@ -89,4 +89,10 @@ extern "C" {
     pub fn b200_encoder_compress_range(e: *mut B200Encoder, quality: i32, lgwin: i32, size_hint: u64, input: *const u8, n: usize,
                                        range_start: usize, range_len: usize, first: i32, last: i32, byte_align: i32, out: *mut u8,
                                        out_cap: usize, out_size: *mut usize, device_io: i32) -> i32;
+    pub fn b200_encoder_reserve(e: *mut B200Encoder, quality: i32, lgwin: i32, size_hint: u64, n: usize, range_len: usize) -> i32;
+    /// `input`, `out` and `out_size` are device pointers; `stream` is a `cudaStream_t` (null = the legacy default stream).
+    pub fn b200_encoder_compress_range_async(e: *mut B200Encoder, quality: i32, lgwin: i32, size_hint: u64, input: *const u8,
+                                             n: usize, range_start: usize, range_len: usize, first: i32, last: i32,
+                                             byte_align: i32, out: *mut u8, out_cap: usize, out_size: *mut u64,
+                                             stream: *mut c_void) -> i32;
 }
