@@ -1,8 +1,9 @@
 /* brotli_b200.h -- C ABI of the GPU-native (CUDA, H100) brotli compression path.
  *
  * This library is a drop-in for the COMPRESSION entry points that the reference (dropbox/rust-brotli 8.0.4)
- * exports from its cdylib; each declaration cites the reference interface it replaces.  Decompression, the
- * BroCatli concatenator and the CLI are out of scope (SURVEY.md section 8).  All pointers are plain host
+ * exports from its cdylib; each declaration cites the reference interface it replaces.  The reference's stream concatenator
+ * (Broccoli) is declared in broccoli.h; its device counterpart b200_concat_async is below.  Decompression and the CLI are out of
+ * scope (SURVEY.md section 8).  All pointers are plain host
  * pointers unless a function says otherwise; no CUDA or torch types appear in any signature.
  *
  * Failure behaviour mirrors the reference: functions return BROTLI_FALSE / NULL / 0 on any error (including
@@ -186,7 +187,38 @@ int b200_encoder_reserve(B200Encoder* e, int quality, int lgwin, uint64_t size_h
 int b200_encoder_compress_range_async(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n,
                                       size_t range_start, size_t range_len, int first, int last, int byte_align, uint8_t* out,
                                       size_t out_cap, uint64_t* out_size, void* stream);
+/* One complete stream of the n device bytes at `in`, with the key / value parameters of BrotliEncoderCompressMulti (the same
+ * parameters are refused; the call then enqueues nothing).  For n < 1 GiB (larger n is refused) the bytes equal those of
+ * BrotliEncoderCompressStream called once with the whole input and BROTLI_OPERATION_FINISH, with the same parameters: the
+ * size hint is SIZE_HINT, or n; every framing mode (CATABLE, APPENDABLE, MAGIC_NUMBER, BYTE_ALIGN, BARE_STREAM) is produced.
+ * NO_DICTIONARY, DISABLE_LITERAL_CONTEXT_MODELING and catable's "no static dictionary" apply to this call only: the encoder's
+ * options are as they were before.  Ordering, output, refusals (out_cap < b200_max_compressed_size(n) + 64, ...), reservation
+ * (b200_encoder_reserve with the same quality, lgwin, size hint and n) and graph capture: as b200_encoder_compress_range_async.
+ * The prologue of a framed stream (window bits, magic-number metadata block, the catable stream's first two bytes as an
+ * uncompressed metablock; <= 24 bytes) is written by a kernel from host-known bits passed as kernel parameters; a stream of at
+ * most two bytes (or empty) is prologue and trailer only and uses no encoder workspace. */
+int b200_encoder_compress_params_async(B200Encoder* e, size_t num_params, const BrotliEncoderParameter* keys, const uint32_t* values,
+                                       const uint8_t* in, size_t n, uint8_t* out, size_t out_cap, uint64_t* out_size, void* stream);
 int b200_encoder_last_timings(B200Encoder* e, float* ms, uint32_t* launches);
+
+/* ---- device splice of catable streams (the reference's BroCatli, src/concat/mod.rs; host ABI in broccoli.h) ---- */
+/* Bytes of device workspace b200_concat_async needs for `count` streams. */
+size_t b200_concat_workspace_size(uint32_t count);
+/* Splices `count` device-resident streams into one, stream-ordered on `stream` (a cudaStream_t as void*).  d_streams[i] (device
+ * array of device pointers) holds d_sizes[i] bytes (device array): the sizes are read on the device, so sizes written by
+ * b200_encoder_compress_range_async earlier on `stream` need no host synchronisation.  out, d_out_size, d_result[2] and
+ * d_workspace (>= b200_concat_workspace_size(count) bytes) are device memory.
+ *  - Result: out[0, *d_out_size) and d_result equal the host sequence window_size ? BroccoliCreateInstanceWithWindowSize(window_size)
+ *    : BroccoliCreateInstance(), then per stream BroccoliNewBrotliFile + BroccoliConcatStream over all of its bytes with unbounded
+ *    output, then BroccoliConcatFinish.  d_result = {0, -1} on success.
+ *  - All or nothing: on the first stream whose ConcatStream fails, d_result = {code (124..127), stream index}; when the output
+ *    would pass out_cap, {2, index of the first stream that does not fit, or count for the final bytes}.  Then *d_out_size = 0
+ *    and nothing is written to out.
+ *  - Size: the output never exceeds the sum of the sizes + 3 bytes (derivation in csrc/bro_concat.cuh); offsets are 64-bit.
+ *  - Allocates nothing, never waits on the host and is capturable in a CUDA graph: four launches and one memset on `stream`.
+ *    Returns 0 (nothing enqueued) for null pointers, a short workspace, count > 2^31 - 1 or window_size outside 0..255. */
+int b200_concat_async(const uint8_t* const* d_streams, const uint64_t* d_sizes, uint32_t count, int window_size, uint8_t* out,
+                      size_t out_cap, uint64_t* d_out_size, int32_t* d_result, void* d_workspace, size_t workspace_bytes, void* stream);
 /* stage hook of quality 5..9: best[] of the match stage (distance << 8 | capped length, or a static-dictionary candidate) for
  * [range_start, range_start + range_len) of an n-byte buffer, range_len <= one chunk; size_hint 0 = n.  search = 0: the up-front
  * kernels; search = 1: the on-demand search at every position (returns 0 where that path does not run: depth < 64, two batches) */

@@ -132,13 +132,17 @@ def encoder_compress(data: bytes, quality: int = 11, lgwin: int = 22) -> bytes:
 _tensor_encoders = {}  # CUDA ordinal -> the DeviceEncoder compress_tensor uses when it is given none
 
 
-def compress_tensor(t, quality: int = 5, lgwin: int = 22, encoder: DeviceEncoder = None):
+def compress_tensor(t, quality: int = 5, lgwin: int = 22, encoder: DeviceEncoder = None, params: BrotliEncoderParams = None):
     """Compresses a contiguous uint8 CUDA tensor on ``torch.cuda.current_stream()`` without waiting for it.
 
     Returns ``(out, size)``: a uint8 tensor of capacity bytes whose first ``size`` bytes become the brotli stream, and a
     one-element int64 tensor holding that size, both on ``t``'s device and both written in the order of the current stream (read
     them after it, e.g. ``out[:size.item()]``, which synchronises).  Nothing here synchronises.  Inside ``torch.cuda.graph``
     pass an ``encoder`` on which ``reserve(quality, lgwin, t.numel())`` was called before the capture.
+
+    With ``params`` (``quality`` and ``lgwin`` are then taken from it) the stream is the one ``BrotliEncoderCompressStream`` with
+    these parameters and one FINISH produces (``b200_encoder_compress_params_async``), framing included: streams made with
+    ``catable=True`` can be spliced on the device by ``concat_tensors``.
     """
     import torch
     if not (t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
@@ -155,8 +159,130 @@ def compress_tensor(t, quality: int = 5, lgwin: int = 22, encoder: DeviceEncoder
     out = torch.empty(cap, dtype=torch.uint8, device=t.device)
     size = torch.empty(1, dtype=torch.int64, device=t.device)
     stream = torch.cuda.current_stream(t.device)
-    encoder.compress_async(t.data_ptr(), n, out.data_ptr(), cap, size.data_ptr(), quality, lgwin, stream.cuda_stream)
+    if params is not None:
+        encoder.compress_params_async(t.data_ptr(), n, out.data_ptr(), cap, size.data_ptr(), params.as_key_values(), stream.cuda_stream)
+    else:
+        encoder.compress_async(t.data_ptr(), n, out.data_ptr(), cap, size.data_ptr(), quality, lgwin, stream.cuda_stream)
     return out, size
+
+
+# BroccoliResult / BroCatliResult (src/concat/mod.rs:3-13)
+BROCCOLI_SUCCESS, BROCCOLI_NEEDS_MORE_INPUT, BROCCOLI_NEEDS_MORE_OUTPUT = 0, 1, 2
+BROCCOLI_NOT_CRAFTED_FOR_APPEND, BROCCOLI_INVALID_WINDOW_SIZE = 124, 125
+BROCCOLI_WINDOW_SIZE_LARGER_THAN_PREVIOUS_FILE, BROCCOLI_NOT_CRAFTED_FOR_CONCATENATION = 126, 127
+
+
+class BroccoliState(ctypes.Structure):
+    """include/broccoli.h: the whole splice state, plain data."""
+    _fields_ = [("unused", ctypes.c_void_p), ("data", ctypes.c_ubyte * 248)]
+
+
+def _broccoli():
+    L = lib()
+    if not getattr(L, "_broccoli_ready", False):
+        sz, P = ctypes.c_size_t, ctypes.POINTER
+        L.BroccoliCreateInstance.restype = BroccoliState
+        L.BroccoliCreateInstance.argtypes = []
+        L.BroccoliCreateInstanceWithWindowSize.restype = BroccoliState
+        L.BroccoliCreateInstanceWithWindowSize.argtypes = [ctypes.c_uint8]
+        L.BroccoliNewBrotliFile.argtypes = [P(BroccoliState)]
+        L.BroccoliNewBrotliFile.restype = None
+        L.BroccoliConcatStreaming.argtypes = [P(BroccoliState), P(sz), ctypes.c_void_p, P(sz), ctypes.c_void_p]
+        L.BroccoliConcatStreaming.restype = ctypes.c_int
+        L.BroccoliConcatFinished.argtypes = [P(BroccoliState), P(sz), ctypes.c_void_p]
+        L.BroccoliConcatFinished.restype = ctypes.c_int
+        L.b200_concat_workspace_size.argtypes = [ctypes.c_uint32]
+        L.b200_concat_workspace_size.restype = sz
+        L.b200_concat_async.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32, ctypes.c_int, ctypes.c_void_p, sz,
+                                        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, sz, ctypes.c_void_p]
+        L.b200_concat_async.restype = ctypes.c_int
+        L._broccoli_ready = True
+    return L
+
+
+class BroCatli:
+    """The reference's stream stitcher (src/concat/mod.rs ``BroCatli``) over the Broccoli C ABI (include/broccoli.h).
+
+    ``new_brotli_file()`` starts the next stream; ``stream(data, out_cap)`` feeds it and ``finish(out_cap)`` ends the spliced
+    stream.  Both return ``(result, consumed, output)`` / ``(result, output)`` with at most ``out_cap`` output bytes, as one call of
+    the reference does over buffers of those sizes.  Host code: no CUDA device is needed."""
+
+    def __init__(self, _state=None):
+        self._L = _broccoli()
+        self._s = self._L.BroccoliCreateInstance() if _state is None else _state
+
+    @classmethod
+    def new_with_window_size(cls, window_size: int):
+        """An instance that starts as an empty stream of that window; a size the reference refuses gives a default instance."""
+        return cls(_broccoli().BroccoliCreateInstanceWithWindowSize(window_size))
+
+    def new_brotli_file(self):
+        self._L.BroccoliNewBrotliFile(ctypes.byref(self._s))
+
+    def stream(self, data: bytes, out_cap: int):
+        data = bytes(data)
+        avail_in, avail_out = ctypes.c_size_t(len(data)), ctypes.c_size_t(out_cap)
+        obuf = ctypes.create_string_buffer(max(1, out_cap))
+        r = self._L.BroccoliConcatStreaming(ctypes.byref(self._s), ctypes.byref(avail_in), _native._inptr(data),
+                                            ctypes.byref(avail_out), ctypes.cast(obuf, ctypes.c_void_p))
+        return r, len(data) - avail_in.value, obuf.raw[:out_cap - avail_out.value]
+
+    def finish(self, out_cap: int):
+        avail_out = ctypes.c_size_t(out_cap)
+        obuf = ctypes.create_string_buffer(max(1, out_cap))
+        r = self._L.BroccoliConcatFinished(ctypes.byref(self._s), ctypes.byref(avail_out), ctypes.cast(obuf, ctypes.c_void_p))
+        return r, obuf.raw[:out_cap - avail_out.value]
+
+    def state_bytes(self) -> bytes:
+        return bytes(self._s.data)
+
+
+def concat_tensors(parts, window_size: int = 0, pointers=None, workspace=None):
+    """Splices catable streams that live on the GPU into one brotli stream, on ``torch.cuda.current_stream()`` without waiting.
+
+    ``parts`` is a list of ``(out, size)`` pairs as ``compress_tensor`` returns them (``size`` a one-element int64 device tensor,
+    read on the device).  Returns ``(out, size, result)`` device tensors: the spliced stream is ``out[:size]`` and ``result`` holds
+    (BroccoliResult, stream index), both as the host sequence ``BroCatli`` / new_brotli_file + stream per part / finish gives them
+    (``b200_concat_async``).  On failure ``size`` is 0 and ``result`` names the first failing part.
+
+    Inside ``torch.cuda.graph``: the table of stream pointers and the workspace must exist before the capture (building the table
+    copies it from host memory).  Pass ``pointers=concat_pointer_table(parts)`` and
+    ``workspace=torch.empty(concat_workspace_size(len(parts)), dtype=torch.uint8, device=...)`` made outside the capture."""
+    import torch
+    if not parts:
+        raise ValueError("concat_tensors needs at least one part")
+    dev = parts[0][0].device
+    for o, s in parts:
+        if not (o.is_cuda and o.dtype == torch.uint8 and o.device == dev and s.is_cuda and s.dtype == torch.int64 and s.numel() == 1):
+            raise ValueError("parts must be (uint8 CUDA tensor, one-element int64 CUDA tensor) pairs on one device")
+    L = _broccoli()
+    n = len(parts)
+    if pointers is None:
+        pointers = concat_pointer_table(parts)
+    if workspace is None:
+        workspace = torch.empty(L.b200_concat_workspace_size(n), dtype=torch.uint8, device=dev)
+    sizes = torch.cat([s.reshape(1) for _, s in parts])
+    cap = sum(o.numel() for o, _ in parts) + 3  # a part's size is at most its capacity; the splice adds at most 3 bytes
+    out = torch.empty(cap, dtype=torch.uint8, device=dev)
+    size = torch.empty(1, dtype=torch.int64, device=dev)
+    result = torch.empty(2, dtype=torch.int32, device=dev)
+    stream = torch.cuda.current_stream(dev)
+    if not L.b200_concat_async(pointers.data_ptr(), sizes.data_ptr(), n, int(window_size), out.data_ptr(), cap, size.data_ptr(),
+                               result.data_ptr(), workspace.data_ptr(), workspace.numel(), stream.cuda_stream):
+        raise RuntimeError("b200_concat_async refused the call")
+    return out, size, result
+
+
+def concat_pointer_table(parts):
+    """The device table of stream pointers ``concat_tensors`` reads.  It is copied from pinned host memory on the current stream
+    without waiting; being a copy from host memory, it must be built outside a graph capture."""
+    import torch
+    host = torch.tensor([o.data_ptr() for o, _ in parts], dtype=torch.int64).pin_memory()
+    return host.to(parts[0][0].device, non_blocking=True)
+
+
+def concat_workspace_size(count: int) -> int:
+    return _broccoli().b200_concat_workspace_size(count)
 
 
 class _Stream:

@@ -42,6 +42,8 @@ def lib():
         L.b200_encoder_compress_range_async.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.c_uint64, vp, sz, sz, sz, ctypes.c_int,
                                                         ctypes.c_int, ctypes.c_int, vp, sz, vp, vp]
         L.b200_encoder_compress_range_async.restype = ctypes.c_int
+        L.b200_encoder_compress_params_async.argtypes = [vp, sz, vp, vp, vp, sz, vp, sz, vp, vp]
+        L.b200_encoder_compress_params_async.restype = ctypes.c_int
         L.b200_encoder_last_timings.argtypes = [vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_uint32)]
         L.b200_stage_match.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.c_uint64, vp, sz, sz, sz, ctypes.c_int, vp]
         L.b200_stage_match.restype = ctypes.c_int
@@ -137,6 +139,18 @@ class DeviceEncoder:
                                                         ctypes.c_void_p(stream_ptr))
         if not ok:
             raise RuntimeError("b200_encoder_compress_range_async refused the call")
+
+    def compress_params_async(self, d_in_ptr: int, n: int, d_out_ptr: int, out_cap: int, d_size_ptr: int, key_values, stream_ptr: int):
+        """One complete stream of the n device bytes at d_in_ptr with BrotliEncoderCompressMulti-style (key, value) parameters,
+        enqueued on stream_ptr without waiting (b200_encoder_compress_params_async).  Raises if the call is refused."""
+        kv = list(key_values)
+        keys = (ctypes.c_int * max(1, len(kv)))(*[int(k) for k, _ in kv])
+        vals = (ctypes.c_uint32 * max(1, len(kv)))(*[int(v) for _, v in kv])
+        ok = self._L.b200_encoder_compress_params_async(self._h, len(kv), ctypes.cast(keys, ctypes.c_void_p), ctypes.cast(vals, ctypes.c_void_p),
+                                                         ctypes.c_void_p(d_in_ptr), n, ctypes.c_void_p(d_out_ptr), out_cap,
+                                                         ctypes.c_void_p(d_size_ptr), ctypes.c_void_p(stream_ptr))
+        if not ok:
+            raise RuntimeError("b200_encoder_compress_params_async refused the call")
 
     def timings(self):
         ms = (ctypes.c_float * NUM_STAGES)()

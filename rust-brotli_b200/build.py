@@ -7,10 +7,11 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libbrotli_b200.so")
-SOURCES = ["bro_encoder.cu", "bro_capi.cu"]
+SOURCES = ["bro_encoder.cu", "bro_capi.cu", "bro_broccoli.cu", "bro_concat.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper); the TMA bulk copies and mbarriers need sm_90
 DEPS = ["bro_common.cuh", "bro_huffman.cuh", "bro_meta.cuh", "bro_parse.cuh", "bro_split.cuh", "bro_finalize.cuh",
-        "bro_kernels.cuh", "bro_kernels_hq.cuh", "bro_hq.cuh", "bro_bsplit.cuh", "bro_encoder.h", "bro_dict.cuh", "bro_dict_data.inc"]
+        "bro_kernels.cuh", "bro_kernels_hq.cuh", "bro_hq.cuh", "bro_bsplit.cuh", "bro_encoder.h", "bro_dict.cuh", "bro_dict_data.inc",
+        "bro_concat.cuh"]
 
 
 def needs_build():
@@ -18,7 +19,8 @@ def needs_build():
         return True
     t = os.path.getmtime(OUT)
     # this file too: a library built with other flags (another architecture) is stale
-    files = [os.path.join(CSRC, f) for f in SOURCES + DEPS] + [os.path.join(ROOT, "include", "brotli_b200.h"), os.path.abspath(__file__)]
+    files = [os.path.join(CSRC, f) for f in SOURCES + DEPS] + [os.path.join(ROOT, "include", h) for h in ("brotli_b200.h", "broccoli.h")]
+    files.append(os.path.abspath(__file__))
     return any(os.path.exists(f) and os.path.getmtime(f) > t for f in files)
 
 

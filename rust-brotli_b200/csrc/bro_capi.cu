@@ -170,6 +170,45 @@ static void put_window_bits(HostBits& w, int lgwin) {  // EncodeWindowBits encod
   else if (lgwin > 17) w.put(4, (uint64_t)(((lgwin - 17) << 1) | 1));
   else w.put(7, (uint64_t)(((lgwin - 8) << 4) | 1));
 }
+// The prologue of a framed stream of `len` bytes (p sanitised): [window bits unless catable && bare] [magic-number metadata
+// metablock, brotli_bit_stream.rs:2869-2896] [catable: the first min(2, len) bytes as an uncompressed metablock,
+// encode.rs:2285-2333].  data: those first bytes, or nullptr to leave zeros in their place (the device copies them in);
+// *data_off / *n2: where they are and how many.  Shared by compress_framed and b200_encoder_compress_params_async.
+static void write_prologue(HostBits& w, const EncoderParams& p, size_t len, const uint8_t* data, size_t* data_off, size_t* n2) {
+  const int lw = p.lgwin < 10 ? 10 : (p.lgwin > 24 ? 24 : p.lgwin);
+  *data_off = 0;
+  *n2 = 0;
+  if (!(p.catable && p.bare_stream)) put_window_bits(w, lw);
+  if (p.magic_number) {
+    uint8_t sh[10]; size_t nsh = 0;
+    for (uint64_t v = p.size_hint;;) {  // encode_base_128 brotli_bit_stream.rs:2855-2867
+      sh[nsh] = (uint8_t)(v & 0x7f); v >>= 7;
+      if (v) sh[nsh++] |= 0x80; else { ++nsh; break; }
+      if (nsh == 10) break;
+    }
+    w.put(1, 0); w.put(2, 3); w.put(1, 0); w.put(2, 1); w.put(8, 3 + nsh);
+    w.align();
+    const uint8_t magic[4] = {0xe1, 0x97, (uint8_t)(p.catable ? 0x81 : (p.appendable ? 0x82 : 0x80)), 1 /* crate VERSION, lib.rs:67 */};
+    w.bytes(magic, 4);
+    w.bytes(sh, nsh);
+  }
+  if (p.catable && len) {
+    *n2 = std::min<size_t>(2, len);
+    w.put(1, 0); w.put(2, 0); w.put(16, *n2 - 1); w.put(1, 1);  // ISLAST 0, MNIBBLES 4, MLEN - 1, ISUNCOMPRESSED
+    w.align();
+    *data_off = (size_t)(w.pos >> 3);
+    const uint8_t zeros[2] = {0, 0};
+    w.bytes(data ? data : zeros, *n2);
+  }
+}
+// The end of a framed stream with nothing (left) to compress behind the prologue (WriteEmptyLastBlocksInternal
+// encode.rs:1928-1940): last: [byte_align: padding metablock][unless bare: the empty last metablock]; else padding if asked.
+static void write_empty_trailer(HostBits& w, const EncoderParams& p, bool last, bool align_end) {
+  if (last) {
+    if (p.byte_align && (w.pos & 7)) { w.put(6, 6); w.align(); }  // BrotliWritePaddingMetaBlock
+    if (!p.bare_stream) { w.put(2, 3); w.align(); }
+  } else if (align_end && (w.pos & 7)) { w.put(6, 6); w.align(); }
+}
 // Compresses input[a, b) like compress_span and wraps it in the framing `p` asks for:
 //   first: [window bits unless catable && bare] [magic-number metadata metablock, brotli_bit_stream.rs:2869-2896]
 //          [catable: the first min(2, len) bytes as an uncompressed metablock, encode.rs:2285-2333 -- a stitched stream's literal
@@ -181,33 +220,14 @@ static bool compress_framed(B200Encoder* enc, EncoderParams p, uint64_t hint, co
                             bool last, bool align_end, uint8_t* out, size_t out_cap, size_t* out_size) {
   sanitize_framing(p);
   if (!framed(p)) return compress_span(enc, p, hint, input, a, b, first, last, align_end, out, out_cap, out_size);
-  const int lw = p.lgwin < 10 ? 10 : (p.lgwin > 24 ? 24 : p.lgwin);
   HostBits w{out, out_cap};
   size_t body_a = a;
   bool dev_first = first;
   if (first && (p.magic_number || p.catable || a == b)) {
     dev_first = false;
-    if (!(p.catable && p.bare_stream)) put_window_bits(w, lw);
-    if (p.magic_number) {
-      uint8_t sh[10]; size_t nsh = 0;
-      for (uint64_t v = p.size_hint;;) {  // encode_base_128 brotli_bit_stream.rs:2855-2867
-        sh[nsh] = (uint8_t)(v & 0x7f); v >>= 7;
-        if (v) sh[nsh++] |= 0x80; else { ++nsh; break; }
-        if (nsh == 10) break;
-      }
-      w.put(1, 0); w.put(2, 3); w.put(1, 0); w.put(2, 1); w.put(8, 3 + nsh);
-      w.align();
-      const uint8_t magic[4] = {0xe1, 0x97, (uint8_t)(p.catable ? 0x81 : (p.appendable ? 0x82 : 0x80)), 1 /* crate VERSION, lib.rs:67 */};
-      w.bytes(magic, 4);
-      w.bytes(sh, nsh);
-    }
-    if (p.catable && b > a) {
-      const size_t n2 = std::min<size_t>(2, b - a);
-      w.put(1, 0); w.put(2, 0); w.put(16, n2 - 1); w.put(1, 1);  // ISLAST 0, MNIBBLES 4, MLEN - 1, ISUNCOMPRESSED
-      w.align();
-      w.bytes(input + a, n2);
-      body_a += n2;
-    }
+    size_t data_off, n2;
+    write_prologue(w, p, b - a, input + a, &data_off, &n2);
+    body_a += n2;
   }
   if (!w.ok) return false;
   size_t off = (size_t)(w.pos >> 3);
@@ -227,10 +247,7 @@ static bool compress_framed(B200Encoder* enc, EncoderParams p, uint64_t hint, co
     return true;
   }
   // nothing (left) to compress: the trailer follows the prologue directly
-  if (last) {
-    if (p.byte_align && (w.pos & 7)) { w.put(6, 6); w.align(); }  // BrotliWritePaddingMetaBlock
-    if (!p.bare_stream) { w.put(2, 3); w.align(); }
-  } else if (align_end && (w.pos & 7)) { w.put(6, 6); w.align(); }
+  write_empty_trailer(w, p, last, align_end);
   if (!w.ok || (w.pos & 7)) return false;
   *out_size = (size_t)(w.pos >> 3);
   return true;
@@ -434,6 +451,48 @@ BROTLI_BOOL BrotliEncoderCompress(int quality, int lgwin, BrotliEncoderMode mode
   }
   *encoded_size = got;
   return BROTLI_TRUE;
+}
+
+// One complete stream of the n device bytes at `in`, stream-ordered on `stream`: the bytes of compress_framed(first, last) --
+// which BrotliEncoderCompressStream with one FINISH runs -- with the prologue written by a kernel and the body compressed behind it.
+int b200_encoder_compress_params_async(B200Encoder* e, size_t num_params, const BrotliEncoderParameter* keys, const uint32_t* values,
+                                       const uint8_t* in, size_t n, uint8_t* out, size_t out_cap, uint64_t* out_size, void* stream) {
+  if (!e || (num_params && (!keys || !values))) return 0;
+  if (n >= kSpanPiece) return 0;  // one span piece: longer inputs are cut into pieces by compress_span
+  if (out_cap < b200_max_compressed_size(n) + 64) return 0;
+  EncoderParams p;
+  for (size_t i = 0; i < num_params; ++i)
+    if (!apply_param(p, (int)keys[i], values[i])) return 0;
+  sanitize_framing(p);
+  const uint64_t hint = p.size_hint ? p.size_hint : n;
+  const int ctx = p.disable_ctx ? 0 : 1, dict = p.no_dictionary ? 0 : 1;
+  if (!framed(p))
+    return b200_encoder_compress_framed_async(e, p.quality, p.lgwin, hint, ctx, dict, in, n, 0, n, 1, 1, 0, nullptr, -1, out, out_cap,
+                                              out_size, stream);
+  B200Prologue pro;
+  memset(&pro, 0, sizeof(pro));
+  HostBits w{pro.bytes, sizeof(pro.bytes)};
+  size_t body_a = 0, data_off = 0, n2 = 0;
+  const bool has_prologue = p.magic_number || p.catable || n == 0;
+  if (has_prologue) write_prologue(w, p, n, nullptr, &data_off, &n2);
+  body_a = n2;
+  if (!w.ok) return 0;
+  pro.data_off = (uint32_t)data_off;
+  pro.n2 = (uint32_t)n2;
+  if (body_a < n) {  // as compress_framed: the device writes the plain trailer itself unless the stream ends byte aligned
+    if (w.pos & 7) return 0;
+    pro.len = (uint32_t)(w.pos >> 3);
+    const bool dev_last = !p.byte_align && !p.bare_stream;
+    return b200_encoder_compress_framed_async(e, p.quality, p.lgwin, hint, ctx, dict, in, n, body_a, n - body_a, has_prologue ? 0 : 1,
+                                              dev_last ? 1 : 0, p.byte_align ? 1 : 0, has_prologue ? &pro : nullptr,
+                                              (p.byte_align && !p.bare_stream) ? 3 : -1, out, out_cap, out_size, stream);
+  }
+  write_empty_trailer(w, p, true, true);
+  if (!w.ok || (w.pos & 7)) return 0;
+  pro.len = (uint32_t)(w.pos >> 3);
+  pro.complete = 1;
+  return b200_encoder_compress_framed_async(e, p.quality, p.lgwin, hint, ctx, dict, in, n, n, 0, 0, 0, 0, &pro, -1, out, out_cap,
+                                            out_size, stream);
 }
 
 // ---- multi ----

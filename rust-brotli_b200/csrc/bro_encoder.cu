@@ -767,13 +767,18 @@ size_t b200_max_compressed_size(size_t n) { return n + (n >> 10) * 8 + 4096; }
 // each chunk's end bit position is copied to h_total[k] on its lane and h_done[k] is recorded behind it.
 //
 // Pipeline: the input is staged chunk by chunk on a copy stream and chunks alternate between the compute lanes.
+// pro (device input only): the prologue of a framed stream goes in front, and the first chunk starts behind it.
 static bool enqueue_range(B200Encoder* e, const CallPlan& c, const uint8_t* in, cudaMemcpyKind in_kind, uint8_t* out, bool first,
-                          bool last, bool byte_align, std::vector<cudaEvent_t>* h_done) {
+                          bool last, bool byte_align, std::vector<cudaEvent_t>* h_done, const B200Prologue* pro = nullptr) {
   const size_t nchunks = c.chunks.size();
   e->data_base = c.base;
   uint8_t* dd = e->d_data.as<uint8_t>();
   CUDA_OK(cudaMemsetAsync(out, 0, c.need, e->s_in));
   CUDA_OK(cudaMemsetAsync(e->d_total.p, 0, 8, e->s_in));
+  if (pro) {
+    k_prologue<<<1, 32, 0, e->s_in>>>(*pro, in, out, e->d_total.as<uint64_t>(), nullptr);
+    e->launches += 1;
+  }
   CUDA_OK(cudaMemsetAsync(dd + c.staged, 0, kPad, e->s_in));
   cudaEvent_t prev_layout = nullptr;
   size_t copied = c.base;  // absolute position up to which the input is staged
@@ -853,14 +858,15 @@ static bool compress_range_impl(B200Encoder* e, int quality, int lgwin, uint64_t
 // into the lanes), joins back into `st` behind the last work of s_in and of every lane it used, and writes *out_size with one
 // more launch on `st`.  Inside a capture it neither waits for nor records ev_call: a graph may not depend on work outside it.
 static bool enqueue_async(B200Encoder* e, const CallPlan& c, const uint8_t* in, bool first, bool last, bool byte_align,
-                          bool empty_stream, uint8_t* out, uint64_t* out_size, cudaStream_t st, bool capturing) {
+                          bool empty_stream, uint8_t* out, uint64_t* out_size, cudaStream_t st, bool capturing,
+                          const B200Prologue* pro = nullptr, int trailer = -1) {
   const size_t nchunks = c.chunks.size();
   cudaEvent_t fork = e->sync_events.get(false);
   CUDA_OK(cudaEventRecord(fork, st));
   CUDA_OK(cudaStreamWaitEvent(e->s_in, fork, 0));
   if (!capturing) CUDA_OK(cudaStreamWaitEvent(e->s_in, e->ev_call, 0));
   if (nchunks) {
-    if (!enqueue_range(e, c, in, cudaMemcpyDeviceToDevice, out, first, last, byte_align, nullptr)) return false;
+    if (!enqueue_range(e, c, in, cudaMemcpyDeviceToDevice, out, first, last, byte_align, nullptr, pro)) return false;
   } else {
     CUDA_OK(cudaMemsetAsync(out, 0, c.need, e->s_in));
   }
@@ -873,7 +879,7 @@ static bool enqueue_async(B200Encoder* e, const CallPlan& c, const uint8_t* in, 
     CUDA_OK(cudaEventRecord(join, used[i]));
     CUDA_OK(cudaStreamWaitEvent(st, join, 0));
   }
-  k_out_size<<<1, 1, 0, st>>>(nchunks ? e->d_total.as<uint64_t>() + nchunks : nullptr, out, empty_stream ? 1 : 0, out_size);
+  k_out_size<<<1, 1, 0, st>>>(nchunks ? e->d_total.as<uint64_t>() + nchunks : nullptr, out, empty_stream ? 1 : 0, out_size, trailer);
   e->launches += 1;
   CUDA_OK(cudaGetLastError());
   if (!capturing) CUDA_OK(cudaEventRecord(e->ev_call, st));
@@ -908,17 +914,20 @@ int b200_encoder_reserve(B200Encoder* e, int quality, int lgwin, uint64_t size_h
   return e->provide(s, true) ? 1 : 0;
 }
 
-int b200_encoder_compress_range_async(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n,
-                                      size_t range_start, size_t range_len, int first, int last, int byte_align, uint8_t* out,
-                                      size_t out_cap, uint64_t* out_size, void* stream) {
+// b200_encoder_compress_range_async and, with a prologue / trailer / per-call options, b200_encoder_compress_framed_async
+static int compress_async_impl(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, int ctx_model, int use_dict,
+                               const uint8_t* in, size_t n, size_t range_start, size_t range_len, int first, int last, int byte_align,
+                               const B200Prologue* pro, int trailer, uint8_t* out, size_t out_cap, uint64_t* out_size, void* stream) {
   if (!e || !e->ok || !out || !out_size) return 0;
   if (n >= 0xFFFFF000ull || range_start > n || range_len > n - range_start) return 0;  // 32-bit positions
+  if (pro && (pro->len > sizeof(pro->bytes) || pro->data_off + pro->n2 > pro->len || pro->n2 > n)) return 0;
   if (cudaSetDevice(e->device) != cudaSuccess) return 0;
   if (out_cap < b200_max_compressed_size(range_len) + 64 || (reinterpret_cast<uintptr_t>(out) & 3)) return 0;
+  const bool reads_in = range_len || (pro && pro->n2);
   // (the pointer queries run in relaxed capture mode: under a global-mode capture on another stream they are no reason to fail)
   cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
   if (cudaThreadExchangeStreamCaptureMode(&mode) != cudaSuccess) return 0;
-  const bool placed = on_device(out, e->device) && on_device(out_size, e->device) && (!range_len || on_device(in, e->device));
+  const bool placed = on_device(out, e->device) && on_device(out_size, e->device) && (!reads_in || on_device(in, e->device));
   cudaThreadExchangeStreamCaptureMode(&mode);
   if (!placed) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -929,8 +938,18 @@ int b200_encoder_compress_range_async(B200Encoder* e, int quality, int lgwin, ui
   }
   if (cs == cudaStreamCaptureStatusInvalidated) return 0;
   const bool capturing = cs == cudaStreamCaptureStatusActive;
+  if (pro && pro->complete) {  // the whole stream is prologue and trailer: nothing of the encoder is used
+    k_prologue<<<1, 32, 0, st>>>(*pro, in, out, nullptr, out_size);
+    return cudaGetLastError() == cudaSuccess ? 1 : 0;
+  }
+  const int saved_ctx = e->ctx_model, saved_dict = e->use_dict;
+  if (ctx_model >= 0) e->ctx_model = ctx_model;  // read into the call's parameters by plan_call, restored below
+  if (use_dict >= 0) e->use_dict = use_dict;
   CallPlan c;
   e->plan_call(&c, quality, lgwin, size_hint ? size_hint : n, range_start, range_len);
+  e->ctx_model = saved_ctx;
+  e->use_dict = saved_dict;
+  if (pro && c.chunks.empty()) return 0;  // a prologue in front of nothing is a complete one
   if (!e->provide(e->sizes_of(c), !capturing)) {
     if (capturing) fprintf(stderr, "[brotli_b200] a call inside a CUDA graph capture needs b200_encoder_reserve first\n");
     return 0;
@@ -942,13 +961,28 @@ int b200_encoder_compress_range_async(B200Encoder* e, int quality, int lgwin, ui
   const bool timing = e->timing;
   e->timing = false;  // stage timing would read events back on the host
   const bool ok = enqueue_async(e, c, in, first != 0, last != 0, byte_align != 0, first && last && n == 0, out, out_size, st,
-                                capturing);
+                                capturing, pro, trailer);
   e->timing = timing;
   if (!ok) {
     if (!capturing) cudaDeviceSynchronize();  // leave no work in flight behind a failed call
     return 0;
   }
   return 1;
+}
+
+int b200_encoder_compress_range_async(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n,
+                                      size_t range_start, size_t range_len, int first, int last, int byte_align, uint8_t* out,
+                                      size_t out_cap, uint64_t* out_size, void* stream) {
+  return compress_async_impl(e, quality, lgwin, size_hint, -1, -1, in, n, range_start, range_len, first, last, byte_align, nullptr, -1,
+                             out, out_cap, out_size, stream);
+}
+
+int b200_encoder_compress_framed_async(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, int ctx_model, int use_dict,
+                                       const uint8_t* in, size_t n, size_t range_start, size_t range_len, int first, int last,
+                                       int byte_align, const B200Prologue* pro, int trailer, uint8_t* out, size_t out_cap,
+                                       uint64_t* out_size, void* stream) {
+  return compress_async_impl(e, quality, lgwin, size_hint, ctx_model, use_dict, in, n, range_start, range_len, first, last, byte_align,
+                             pro, trailer, out, out_cap, out_size, stream);
 }
 
 int b200_encoder_compress_range(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n,

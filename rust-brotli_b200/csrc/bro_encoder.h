@@ -25,6 +25,20 @@ int b200_encoder_reserve(B200Encoder* e, int quality, int lgwin, uint64_t size_h
 int b200_encoder_compress_range_async(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n,
                                       size_t range_start, size_t range_len, int first, int last, int byte_align, uint8_t* out,
                                       size_t out_cap, uint64_t* out_size, void* stream);
+/* Framed stream-ordered compression (b200_encoder_compress_params_async builds on it).  The prologue of a framed stream (window
+ * bits, magic-number metadata block, catable uncompressed metablock -- bro_capi.cu:write_prologue) as built on the host: `len`
+ * bytes, of which [data_off, data_off + n2) are placeholders for the first n2 input bytes.  complete: the prologue is the whole
+ * stream (nothing left to compress, trailer included). */
+typedef struct B200Prologue {
+  uint8_t bytes[32];
+  uint32_t len, data_off, n2, complete;
+} B200Prologue;
+/* b200_encoder_compress_range_async behind a prologue: the range's first metablock starts at byte pro->len (pro may be NULL), and
+ * trailer >= 0 appends that byte behind the range's byte-aligned end.  ctx_model / use_dict apply to this call only. */
+int b200_encoder_compress_framed_async(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, int ctx_model, int use_dict,
+                                       const uint8_t* in, size_t n, size_t range_start, size_t range_len, int first, int last,
+                                       int byte_align, const B200Prologue* pro, int trailer, uint8_t* out, size_t out_cap,
+                                       uint64_t* out_size, void* stream);
 int b200_encoder_last_timings(B200Encoder* e, float* ms /* [B200_NUM_STAGES] */, uint32_t* launches);
 int b200_stage_match(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n, size_t range_start,
                      size_t range_len, int search, uint32_t* best_out);

@@ -17,6 +17,7 @@
 #include <stdint.h>
 
 #include "bro_common.cuh"
+#include "bro_encoder.h"
 #include "bro_finalize.cuh"
 #include "bro_huffman.cuh"
 #include "bro_meta.cuh"
@@ -2275,14 +2276,28 @@ __global__ void k_layout(Workspace W, int first, int last, int byte_align, uint6
 
 // Single thread, last launch of a stream-ordered call: the byte size of the range's output, from the end bit position of its last
 // chunk (end_bits), or -- a call without chunks -- of the empty stream (encode.rs:1463-1467: one byte 6) or of nothing.
-__global__ void k_out_size(const uint64_t* end_bits, uint8_t* out, int empty_stream, uint64_t* out_size) {
+// trailer >= 0: one more byte behind the (byte-aligned) end, the ISLAST + ISLASTEMPTY byte of a byte-aligned framed stream.
+__global__ void k_out_size(const uint64_t* end_bits, uint8_t* out, int empty_stream, uint64_t* out_size, int trailer) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   if (end_bits) {
-    *out_size = (*end_bits + 7) >> 3;
+    uint64_t n = (*end_bits + 7) >> 3;
+    if (trailer >= 0) out[n++] = (uint8_t)trailer;
+    *out_size = n;
     return;
   }
   if (empty_stream) out[0] = 6;
   *out_size = empty_stream ? 1 : 0;
+}
+
+// Single thread: the host-built prologue of a framed stream (B200Prologue, bro_capi.cu:write_prologue) into out, its data bytes
+// (the first n2 input bytes of a catable stream) taken from `in`.  Then either the chunks continue behind it (total_bits = its
+// bit length, so k_layout of the first chunk starts there) or, when it is the whole stream, its size goes to out_size.
+__global__ void k_prologue(B200Prologue pro, const uint8_t* in, uint8_t* out, uint64_t* total_bits, uint64_t* out_size) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  for (uint32_t i = 0; i < pro.len; ++i) out[i] = pro.bytes[i];
+  for (uint32_t i = 0; i < pro.n2; ++i) out[pro.data_off + i] = in[i];
+  if (total_bits) *total_bits = 8ull * pro.len;
+  if (out_size) *out_size = pro.len;
 }
 
 __global__ void __launch_bounds__(256) k_emit_header(Workspace W) {

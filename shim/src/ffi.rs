@@ -95,4 +95,42 @@ extern "C" {
                                              n: usize, range_start: usize, range_len: usize, first: i32, last: i32,
                                              byte_align: i32, out: *mut u8, out_cap: usize, out_size: *mut u64,
                                              stream: *mut c_void) -> i32;
+    /// `input`, `out` and `out_size` are device pointers; `keys` / `values` are host arrays of `num_params` entries.
+    pub fn b200_encoder_compress_params_async(e: *mut B200Encoder, num_params: usize, keys: *const u32, values: *const u32,
+                                              input: *const u8, n: usize, out: *mut u8, out_cap: usize, out_size: *mut u64,
+                                              stream: *mut c_void) -> i32;
+    pub fn b200_concat_workspace_size(count: u32) -> usize;
+    /// Every pointer is a device pointer; `stream` is a `cudaStream_t`.
+    pub fn b200_concat_async(streams: *const *const u8, sizes: *const u64, count: u32, window_size: i32, out: *mut u8,
+                             out_cap: usize, out_size: *mut u64, result: *mut i32, workspace: *mut c_void, workspace_bytes: usize,
+                             stream: *mut c_void) -> i32;
+    // ---- src/ffi/broccoli.rs (include/broccoli.h) ----
+    pub fn BroccoliCreateInstance() -> BroccoliState;
+    pub fn BroccoliCreateInstanceWithWindowSize(window_size: u8) -> BroccoliState;
+    pub fn BroccoliDestroyInstance(state: BroccoliState);
+    pub fn BroccoliNewBrotliFile(state: *mut BroccoliState);
+    pub fn BroccoliConcatStream(state: *mut BroccoliState, available_in: *mut usize, input_buf_ptr: *mut *const u8,
+                                available_out: *mut usize, output_buf_ptr: *mut *mut u8) -> BroccoliResult;
+    pub fn BroccoliConcatStreaming(state: *mut BroccoliState, available_in: *mut usize, input_buf: *const u8,
+                                   available_out: *mut usize, output_buf: *mut u8) -> BroccoliResult;
+    pub fn BroccoliConcatFinish(state: *mut BroccoliState, available_out: *mut usize, output_buf_ptr: *mut *mut u8) -> BroccoliResult;
+    pub fn BroccoliConcatFinished(state: *mut BroccoliState, available_out: *mut usize, output_buf: *mut u8) -> BroccoliResult;
 }
+
+/// include/broccoli.h: the whole splice state as plain data (`unused` is always null).
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct BroccoliState {
+    pub unused: *mut c_void,
+    pub data: [u8; 248],
+}
+
+/// BroccoliResult (src/concat/mod.rs:3-13); a C enum, passed as an int.
+pub type BroccoliResult = i32;
+pub const BROCCOLI_SUCCESS: BroccoliResult = 0;
+pub const BROCCOLI_NEEDS_MORE_INPUT: BroccoliResult = 1;
+pub const BROCCOLI_NEEDS_MORE_OUTPUT: BroccoliResult = 2;
+pub const BROCCOLI_BROTLI_FILE_NOT_CRAFTED_FOR_APPEND: BroccoliResult = 124;
+pub const BROCCOLI_INVALID_WINDOW_SIZE: BroccoliResult = 125;
+pub const BROCCOLI_WINDOW_SIZE_LARGER_THAN_PREVIOUS_FILE: BroccoliResult = 126;
+pub const BROCCOLI_BROTLI_FILE_NOT_CRAFTED_FOR_CONCATENATION: BroccoliResult = 127;

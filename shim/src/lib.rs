@@ -254,3 +254,45 @@ pub fn compress_multi(params: &BrotliEncoderParams, input: &[u8], output: &mut [
         Err(BrotliEncoderThreadError::OtherThreadPanic) // CUDA failure or a parameter this path does not produce
     }
 }
+
+/// `BroCatli` (src/concat/mod.rs:125-605) over the Broccoli C ABI: `new`, `new_with_window_size`, `new_brotli_file`,
+/// `stream(in, &mut in_offset, out, &mut out_offset)` and `finish(out, &mut out_offset)` with the reference's result codes.
+/// Host code: needs no CUDA device.
+pub struct BroCatli {
+    state: ffi::BroccoliState,
+}
+
+impl Default for BroCatli {
+    fn default() -> Self {
+        Self::new()
+    }
+}
+
+impl BroCatli {
+    pub fn new() -> Self {
+        BroCatli { state: unsafe { ffi::BroccoliCreateInstance() } }
+    }
+    /// A size the reference refuses gives a default instance (broccoli.rs:60-65).
+    pub fn new_with_window_size(log_window_size: u8) -> Self {
+        BroCatli { state: unsafe { ffi::BroccoliCreateInstanceWithWindowSize(log_window_size) } }
+    }
+    pub fn new_brotli_file(&mut self) {
+        unsafe { ffi::BroccoliNewBrotliFile(&mut self.state) }
+    }
+    pub fn stream(&mut self, in_bytes: &[u8], in_offset: &mut usize, out_bytes: &mut [u8], out_offset: &mut usize) -> ffi::BroccoliResult {
+        let input = &in_bytes[*in_offset..];
+        let output = &mut out_bytes[*out_offset..];
+        let (mut avail_in, mut avail_out) = (input.len(), output.len());
+        let r = unsafe { ffi::BroccoliConcatStreaming(&mut self.state, &mut avail_in, input.as_ptr(), &mut avail_out, output.as_mut_ptr()) };
+        *in_offset += input.len() - avail_in;
+        *out_offset += output.len() - avail_out;
+        r
+    }
+    pub fn finish(&mut self, out_bytes: &mut [u8], out_offset: &mut usize) -> ffi::BroccoliResult {
+        let output = &mut out_bytes[*out_offset..];
+        let mut avail_out = output.len();
+        let r = unsafe { ffi::BroccoliConcatFinished(&mut self.state, &mut avail_out, output.as_mut_ptr()) };
+        *out_offset += output.len() - avail_out;
+        r
+    }
+}
