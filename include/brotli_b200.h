@@ -201,6 +201,73 @@ int b200_encoder_compress_params_async(B200Encoder* e, size_t num_params, const 
                                        const uint8_t* in, size_t n, uint8_t* out, size_t out_cap, uint64_t* out_size, void* stream);
 int b200_encoder_last_timings(B200Encoder* e, float* ms, uint32_t* launches);
 
+/* ---- device-resident streams: BrotliEncoderCompressStream with the window, the input and the output on the GPU ---- */
+typedef struct B200Stream B200Stream;
+/* A stream on e's GPU with the key / value parameters of BrotliEncoderCompressMulti (refused as BrotliEncoderSetParameter
+ * refuses them) and, when d_dict is not NULL, the custom dictionary of the dict_len device bytes at d_dict (as
+ * BrotliEncoderSetCustomDictionary after those parameters: the last min(dict_len, 2^lgwin - 16) bytes become window content,
+ * the static dictionary is off).  The dictionary is copied on `stream`: work enqueued there after this call may overwrite it.
+ * dict_len > 0 with a NULL d_dict, or d_dict not device memory of e's GPU, is refused.  e must outlive the stream.  NULL on a
+ * refusal or when memory runs out. */
+B200Stream* b200_stream_create(B200Encoder* e, size_t num_params, const BrotliEncoderParameter* keys, const uint32_t* values,
+                               const uint8_t* d_dict, size_t dict_len, void* stream);
+/* One BrotliEncoderCompressStream step, stream-ordered on `stream` (a cudaStream_t as void*): the n device bytes at d_in are
+ * the new input, op is PROCESS, FLUSH or FINISH.  Returns 1 when the work has been enqueued; nothing on the host waits for it.
+ *  - Bytes: the output of all calls on one stream, appended, equals byte for byte what BrotliEncoderCompressStream outputs for
+ *    the same parameters, the same dictionary and the same sequence of (op, bytes).  The host and this call share one rule for
+ *    when a piece is emitted (PROCESS: a 96 MiB piece whenever two are pending; FLUSH / FINISH: everything pending), its framing
+ *    and size hint, and the window kept in front of it (b200_stage_stream_plan).
+ *  - Input: d_in is copied into the stream's window buffer on `stream`, so work enqueued after the call may overwrite it.
+ *  - Output: each piece is compressed into the stream's scratch buffer; the kernel k_stream_append then reads the piece's size
+ *    and the cursor *d_out_size on the device, copies the piece to out + *d_out_size and advances the cursor.  So out[0,
+ *    *d_out_size) is one contiguous stream over calls; reset *d_out_size to 0 between calls to get the pieces separately.
+ *    *d_status is 0 on success.  A piece that does not fit in out_cap is not written at all and *d_status becomes 2; the stream
+ *    is then failed (its host state has advanced): later calls append nothing and report 2.
+ *  - Ordering: each call forks from `stream` and joins back into it, like b200_encoder_compress_range_async, and calls on one
+ *    encoder run one at a time on the device.  The stream's host state advances when a call is enqueued, so calls on one
+ *    B200Stream must be enqueued in the order they are meant to run (each call also waits, on the device, for the previous one).
+ *  - Refused (0, nothing enqueued): NULL stream / out / d_out_size / d_status, d_in NULL with n > 0, pointers that are not device
+ *    memory of the encoder's GPU, any op after FINISH, EMIT_METADATA, and `stream` capturing a CUDA graph (a replay would not
+ *    advance the host state; the capture stays valid).  After a device failure inside a call (out of memory) the call returns 0
+ *    and the stream is failed.
+ *  - Memory: two window buffers of at most 1.5 x (2^lgwin + 68 KiB + the bytes not yet emitted + n) + 1 MiB each (PROCESS keeps fewer
+ *    than 2 x 96 MiB pending), and an output scratch of b200_max_compressed_size(largest piece) + 128 bytes, pieces being at most
+ *    1 GiB.  They grow when a call needs more, stream-ordered (cudaMallocAsync / cudaFreeAsync on `stream`): growing never waits
+ *    on the host.  The encoder's workspace grows as for b200_encoder_compress_range_async. */
+int b200_stream_compress_async(B200Stream* s, BrotliEncoderOperation op, const uint8_t* d_in, size_t n, uint8_t* out, size_t out_cap,
+                               uint64_t* d_out_size, int32_t* d_status, void* stream);
+/* An upper bound of the bytes b200_stream_compress_async(s, op, ..., n, ...) appends: size `out` by it; 0 for a refused op. */
+size_t b200_stream_output_bound(const B200Stream* s, BrotliEncoderOperation op, size_t n);
+/* Frees the stream's buffers stream-ordered on the CUDA stream of its last call (which must still exist); does not wait. */
+void b200_stream_destroy(B200Stream* s);
+
+/* Counters of one compression stream and the emits of one step (the rule BrotliEncoderCompressStream and b200_stream_* share). */
+typedef struct B200StreamCounters {
+  uint64_t base;          /* stream offset of the first byte still kept (a multiple of 4096); the dictionary starts at 0 */
+  uint64_t flushed;       /* stream offset up to which output has been produced */
+  uint64_t end;           /* stream offset of the end of the input so far */
+  uint64_t dict_len;      /* custom dictionary bytes in front of the input */
+  int32_t header_written; /* the stream header has been emitted */
+  int32_t finished;       /* FINISH has been emitted */
+} B200StreamCounters;
+typedef struct B200StreamEmit {
+  uint64_t start, upto;   /* stream bytes [start, upto) become output (empty for an end-of-stream byte) */
+  uint64_t base;          /* the window base the emit compresses against (its input buffer begins at stream offset base) */
+  uint64_t base_after;    /* the base once the emit is done: bytes in front of it are no longer needed */
+  uint64_t size_hint;
+  int32_t first, last;    /* the emit writes the stream header / ends the stream */
+  int32_t byte;           /* >= 0: the emit's whole output is this byte (6: empty stream; 3: ISLAST + ISLASTEMPTY after a
+                             byte-aligned flush); -1: the framed compression of [start, upto) */
+} B200StreamEmit;
+/* stage hooks of the stream rule (host code, no device needed).  start: the counters of a new stream whose custom dictionary has
+ * dict_size bytes (0: none); *dict_from = index of the first dictionary byte kept.  plan: the emits of one step (op, n new bytes)
+ * from counters *c, and the counters after it.  Both return 0 for a refused parameter; plan also for EMIT_METADATA, an unknown
+ * op, input after FINISH, or more than max_emits emits. */
+int b200_stage_stream_start(size_t num_params, const BrotliEncoderParameter* keys, const uint32_t* values, uint64_t dict_size,
+                            B200StreamCounters* c, uint64_t* dict_from);
+int b200_stage_stream_plan(size_t num_params, const BrotliEncoderParameter* keys, const uint32_t* values, const B200StreamCounters* c,
+                           int op, uint64_t n, B200StreamEmit* emits, size_t max_emits, size_t* num_emits, B200StreamCounters* next);
+
 /* ---- device splice of catable streams (the reference's BroCatli, src/concat/mod.rs; host ABI in broccoli.h) ---- */
 /* Bytes of device workspace b200_concat_async needs for `count` streams. */
 size_t b200_concat_workspace_size(uint32_t count);

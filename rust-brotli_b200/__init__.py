@@ -132,7 +132,26 @@ def encoder_compress(data: bytes, quality: int = 11, lgwin: int = 22) -> bytes:
 _tensor_encoders = {}  # CUDA ordinal -> the DeviceEncoder compress_tensor uses when it is given none
 
 
-def compress_tensor(t, quality: int = 5, lgwin: int = 22, encoder: DeviceEncoder = None, params: BrotliEncoderParams = None):
+def _tensor_encoder(t, encoder):
+    import torch
+    dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
+    if encoder is None:
+        encoder = _tensor_encoders.get(dev)
+        if encoder is None:
+            encoder = _tensor_encoders[dev] = DeviceEncoder(dev)
+    elif encoder.device != dev:
+        raise ValueError("the encoder is on cuda:%d, the tensor on cuda:%d" % (encoder.device, dev))
+    return encoder
+
+
+def _check_tensor(t, what):
+    import torch
+    if not (t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
+        raise ValueError("%s needs a contiguous uint8 CUDA tensor" % what)
+
+
+def compress_tensor(t, quality: int = 5, lgwin: int = 22, encoder: DeviceEncoder = None, params: BrotliEncoderParams = None,
+                    dictionary=None):
     """Compresses a contiguous uint8 CUDA tensor on ``torch.cuda.current_stream()`` without waiting for it.
 
     Returns ``(out, size)``: a uint8 tensor of capacity bytes whose first ``size`` bytes become the brotli stream, and a
@@ -143,17 +162,21 @@ def compress_tensor(t, quality: int = 5, lgwin: int = 22, encoder: DeviceEncoder
     With ``params`` (``quality`` and ``lgwin`` are then taken from it) the stream is the one ``BrotliEncoderCompressStream`` with
     these parameters and one FINISH produces (``b200_encoder_compress_params_async``), framing included: streams made with
     ``catable=True`` can be spliced on the device by ``concat_tensors``.
+
+    With ``dictionary`` (a uint8 CUDA tensor on ``t``'s device) the stream is the one ``BrotliEncoderCompressStream`` makes after
+    ``BrotliEncoderSetCustomDictionary`` with those bytes: a ``DeviceStreamEncoder`` with one FINISH.  Not inside a graph capture.
     """
     import torch
-    if not (t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
-        raise ValueError("compress_tensor needs a contiguous uint8 CUDA tensor")
-    dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
-    if encoder is None:
-        encoder = _tensor_encoders.get(dev)
-        if encoder is None:
-            encoder = _tensor_encoders[dev] = DeviceEncoder(dev)
-    elif encoder.device != dev:
-        raise ValueError("the encoder is on cuda:%d, the tensor on cuda:%d" % (encoder.device, dev))
+    _check_tensor(t, "compress_tensor")
+    encoder = _tensor_encoder(t, encoder)
+    if dictionary is not None:
+        s = DeviceStreamEncoder(params or BrotliEncoderParams(quality=quality, lgwin=lgwin), dictionary=dictionary, encoder=encoder)
+        try:
+            s.finish(t)
+            out, size, _ = s.output()
+        finally:
+            s.close()
+        return out, size
     n = t.numel()
     cap = lib().b200_max_compressed_size(n) + 64
     out = torch.empty(cap, dtype=torch.uint8, device=t.device)
@@ -164,6 +187,96 @@ def compress_tensor(t, quality: int = 5, lgwin: int = 22, encoder: DeviceEncoder
     else:
         encoder.compress_async(t.data_ptr(), n, out.data_ptr(), cap, size.data_ptr(), quality, lgwin, stream.cuda_stream)
     return out, size
+
+
+class DeviceStreamEncoder:
+    """``CompressorWriter`` with tensors in and tensors out: one brotli stream fed incrementally from CUDA tensors, its window (and
+    a custom dictionary) kept on the GPU (``b200_stream_*``).
+
+    ``write(t)`` is a PROCESS step, ``flush()`` a FLUSH (everything written so far becomes decodable output), ``finish()`` ends the
+    stream; ``write`` / ``flush`` / ``finish`` also take a tensor to append first.  The output is appended on the device:
+    ``output()`` returns ``(out, size, status)`` device tensors, the stream so far being ``out[:size]`` and ``status`` 0.  The bytes
+    equal what ``BrotliEncoderCompressStream`` gives for the same parameters, dictionary and sequence of steps.  Everything is
+    enqueued on ``torch.cuda.current_stream()`` and nothing synchronises; steps must be called in the order they are meant to run.
+    ``out`` grows as needed (a new tensor, stream-ordered copy), so take ``output()`` again after each step.  Not inside a graph
+    capture."""
+
+    def __init__(self, params: BrotliEncoderParams = None, dictionary=None, encoder: DeviceEncoder = None, device=None):
+        import torch
+        self._params = params or BrotliEncoderParams()
+        if dictionary is not None:
+            _check_tensor(dictionary, "the dictionary")
+            device = dictionary.device
+        dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        if dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        probe = torch.empty(0, dtype=torch.uint8, device=dev)
+        self._enc = _tensor_encoder(probe, encoder)
+        self._L = lib()
+        self.device = dev
+        n, keys, vals = _native.key_value_arrays(self._params.as_key_values())
+        stream = torch.cuda.current_stream(dev)
+        dptr, dlen = (dictionary.data_ptr(), dictionary.numel()) if dictionary is not None else (0, 0)
+        if dictionary is not None and dlen == 0:  # an empty dictionary still switches the static dictionary off: any non-null
+            self._empty = torch.zeros(1, dtype=torch.uint8, device=dev)  # pointer says so, nothing is read
+            dptr = self._empty.data_ptr()
+        self._h = self._L.b200_stream_create(self._enc._h, n, ctypes.cast(keys, ctypes.c_void_p), ctypes.cast(vals, ctypes.c_void_p),
+                                             ctypes.c_void_p(dptr), dlen, ctypes.c_void_p(stream.cuda_stream))
+        if not self._h:
+            raise ValueError("b200_stream_create refused the parameters or the dictionary")
+        self._out = torch.empty(4096, dtype=torch.uint8, device=dev)
+        self._size = torch.zeros(1, dtype=torch.int64, device=dev)
+        self._status = torch.zeros(1, dtype=torch.int32, device=dev)
+        self._bound = 0  # what the steps so far can have appended at most
+
+    def _step(self, op, t=None):
+        import torch
+        if not self._h:
+            raise ValueError("the stream is closed")
+        if t is None:
+            t = torch.empty(0, dtype=torch.uint8, device=self.device)
+        _check_tensor(t, "DeviceStreamEncoder")
+        if t.device != self.device:
+            raise ValueError("the tensor is on %s, the stream on %s" % (t.device, self.device))
+        n = t.numel()
+        need = self._bound + self._L.b200_stream_output_bound(self._h, op, n)
+        if need > self._out.numel():  # grow the output on the stream: the bytes so far move along
+            out = torch.empty(max(need, 2 * self._out.numel()), dtype=torch.uint8, device=self.device)
+            if self._bound:
+                out[:self._bound].copy_(self._out[:self._bound])
+            self._out = out
+        stream = torch.cuda.current_stream(self.device)
+        if not self._L.b200_stream_compress_async(self._h, op, ctypes.c_void_p(t.data_ptr() if n else 0), n,
+                                                  ctypes.c_void_p(self._out.data_ptr()), self._out.numel(),
+                                                  ctypes.c_void_p(self._size.data_ptr()), ctypes.c_void_p(self._status.data_ptr()),
+                                                  ctypes.c_void_p(stream.cuda_stream)):
+            raise RuntimeError("b200_stream_compress_async refused the call (after finish, or inside a graph capture)")
+        self._bound = need
+
+    def write(self, t):
+        self._step(BROTLI_OPERATION_PROCESS, t)
+        return t.numel()
+
+    def flush(self, t=None):
+        self._step(BROTLI_OPERATION_FLUSH, t)
+
+    def finish(self, t=None):
+        self._step(BROTLI_OPERATION_FINISH, t)
+
+    def output(self):
+        return self._out, self._size, self._status
+
+    def close(self):
+        """Frees the stream's device buffers, stream-ordered behind its last step (no wait)."""
+        if getattr(self, "_h", None):
+            self._L.b200_stream_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 # BroccoliResult / BroCatliResult (src/concat/mod.rs:3-13)

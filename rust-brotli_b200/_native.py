@@ -16,6 +16,18 @@ OPT_HQ_SPLIT, OPT_HQ_UNIT, OPT_ONDEMAND, OPT_HQ_LEVELS = 12, 13, 15, 16
 _lib = None
 
 
+class StreamCounters(ctypes.Structure):
+    """B200StreamCounters (include/brotli_b200.h): the counters of one compression stream."""
+    _fields_ = [("base", ctypes.c_uint64), ("flushed", ctypes.c_uint64), ("end", ctypes.c_uint64), ("dict_len", ctypes.c_uint64),
+                ("header_written", ctypes.c_int32), ("finished", ctypes.c_int32)]
+
+
+class StreamEmit(ctypes.Structure):
+    """B200StreamEmit (include/brotli_b200.h): one emit of a stream step."""
+    _fields_ = [("start", ctypes.c_uint64), ("upto", ctypes.c_uint64), ("base", ctypes.c_uint64), ("base_after", ctypes.c_uint64),
+                ("size_hint", ctypes.c_uint64), ("first", ctypes.c_int32), ("last", ctypes.c_int32), ("byte", ctypes.c_int32)]
+
+
 def lib():
     global _lib
     if _lib is None:
@@ -53,6 +65,20 @@ def lib():
         L.b200_hq_unit.restype = ctypes.c_uint32
         L.b200_stage_sort.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp, sz, ctypes.c_int, vp]
         L.b200_stage_sort.restype = ctypes.c_int
+        L.b200_stream_create.argtypes = [vp, sz, vp, vp, vp, sz, vp]
+        L.b200_stream_create.restype = vp
+        L.b200_stream_compress_async.argtypes = [vp, ctypes.c_int, vp, sz, vp, sz, vp, vp, vp]
+        L.b200_stream_compress_async.restype = ctypes.c_int
+        L.b200_stream_output_bound.argtypes = [vp, ctypes.c_int, sz]
+        L.b200_stream_output_bound.restype = sz
+        L.b200_stream_destroy.argtypes = [vp]
+        L.b200_stream_destroy.restype = None
+        P = ctypes.POINTER
+        L.b200_stage_stream_start.argtypes = [sz, vp, vp, ctypes.c_uint64, P(StreamCounters), P(ctypes.c_uint64)]
+        L.b200_stage_stream_start.restype = ctypes.c_int
+        L.b200_stage_stream_plan.argtypes = [sz, vp, vp, P(StreamCounters), ctypes.c_int, ctypes.c_uint64, P(StreamEmit), sz, P(sz),
+                                             P(StreamCounters)]
+        L.b200_stage_stream_plan.restype = ctypes.c_int
         _lib = L
     return _lib
 
@@ -202,3 +228,32 @@ class DeviceEncoder:
         if not ok:
             raise RuntimeError("b200_stage_sort failed")
         return out
+
+
+def key_value_arrays(key_values):
+    """(count, keys, values) ctypes arrays of (BrotliEncoderParameter, value) pairs, as the C ABI takes them."""
+    kv = list(key_values)
+    keys = (ctypes.c_int * max(1, len(kv)))(*[int(k) for k, _ in kv])
+    vals = (ctypes.c_uint32 * max(1, len(kv)))(*[int(v) for _, v in kv])
+    return len(kv), keys, vals
+
+
+def stream_start(key_values, dict_size: int):
+    """b200_stage_stream_start: (counters, index of the first dictionary byte kept) of a new stream."""
+    n, keys, vals = key_value_arrays(key_values)
+    c, frm = StreamCounters(), ctypes.c_uint64(0)
+    if not lib().b200_stage_stream_start(n, ctypes.cast(keys, ctypes.c_void_p), ctypes.cast(vals, ctypes.c_void_p), dict_size,
+                                         ctypes.byref(c), ctypes.byref(frm)):
+        raise ValueError("b200_stage_stream_start refused the parameters")
+    return c, frm.value
+
+
+def stream_plan(key_values, counters: StreamCounters, op: int, n: int, max_emits: int = 64):
+    """b200_stage_stream_plan: (emits, counters after them) of one stream step, or None when the step is refused."""
+    k, keys, vals = key_value_arrays(key_values)
+    emits = (StreamEmit * max_emits)()
+    count, nxt = ctypes.c_size_t(0), StreamCounters()
+    if not lib().b200_stage_stream_plan(k, ctypes.cast(keys, ctypes.c_void_p), ctypes.cast(vals, ctypes.c_void_p), ctypes.byref(counters),
+                                        op, n, emits, max_emits, ctypes.byref(count), ctypes.byref(nxt)):
+        return None
+    return list(emits[:count.value]), nxt

@@ -98,22 +98,83 @@ B200Encoder* shared_encoder(int device, std::mutex** mu) {
 // Stream state.  Input is buffered on the host; PROCESS turns it into output whenever kStreamPieceBytes are pending (the
 // reference also emits as its blocks fill, encode.rs:2873-2995), FLUSH / FINISH emit whatever is pending.  Pieces end
 // byte aligned (padding metablock), and only the last 2^lgwin bytes in front of the unflushed part are kept as match
-// window, so a stream of any length needs a bounded buffer.
+// window, so a stream of any length needs a bounded buffer.  These decisions are stream_plan's (below), which the device
+// stream (B200Stream) shares.
 constexpr size_t kStreamPieceBytes = (size_t)4 * BRO_CHUNK_BYTES_CAPI;
+
+// The custom dictionary rule (compressor.rs:162 / encode.rs:1205-1260): the last min(size, 2^lgwin - 16) bytes become window
+// content in front of the stream (they occupy positions); a dictionary of at most one byte keeps nothing.  Returns the index
+// of the first byte kept and sets the counters of the new stream.  The caller switches the static dictionary off.
+static uint64_t stream_start(const EncoderParams& p, uint64_t size, B200StreamCounters* c) {
+  memset(c, 0, sizeof(*c));
+  if (size <= 1) return size;
+  const int lw = p.lgwin < 10 ? 10 : (p.lgwin > 24 ? 24 : p.lgwin);
+  const uint64_t keep = std::min<uint64_t>(size, ((uint64_t)1 << lw) - 16);
+  c->dict_len = c->flushed = c->end = keep;
+  return size - keep;
+}
+
+// One step of the stream (BrotliEncoderCompressStream with n new bytes): the emits to run, in order, and the counters after
+// them.  An emit compresses [start, upto) against the bytes from `base` on (compress_framed, align_end) or is one end-of-stream
+// byte; once it is done only the match window in front of the unflushed part is needed, from base_after on.
+static void stream_plan(const EncoderParams& p, const B200StreamCounters& c0, int op, uint64_t n, std::vector<B200StreamEmit>* emits,
+                        B200StreamCounters* next) {
+  EncoderParams fp = p;
+  sanitize_framing(fp);
+  B200StreamCounters c = c0;
+  c.end += n;
+  const int lw = p.lgwin < 10 ? 10 : (p.lgwin > 24 ? 24 : p.lgwin);
+  const uint64_t window = ((uint64_t)1 << lw) + 65536;
+  const uint64_t hint = p.size_hint ? p.size_hint : c.end - c.dict_len;  // the input so far
+  auto emit = [&](bool last, uint64_t upto) {
+    B200StreamEmit m;
+    memset(&m, 0, sizeof(m));
+    m.start = c.flushed;
+    m.upto = upto;
+    m.base = m.base_after = c.base;
+    m.size_hint = hint;
+    m.first = !c.header_written;
+    m.last = last;
+    m.byte = -1;
+    if (upto == c.flushed && !(framed(fp) && m.first)) {  // nothing to compress (only FINISH gets here)
+      if (!last || (!m.first && fp.bare_stream)) return;
+      m.byte = m.first ? 6 : 3;  // empty stream (encode.rs:1463) / ISLAST + ISLASTEMPTY after a byte-aligned flush
+      c.header_written = 1;
+      emits->push_back(m);
+      return;
+    }
+    c.flushed = upto;
+    c.header_written = 1;
+    if (c.flushed > c.base + window) {  // keep only the match window in front of the unflushed part
+      const uint64_t keep_from = (c.flushed - window) & ~(uint64_t)4095;
+      if (keep_from > c.base) c.base = keep_from;
+    }
+    m.base_after = c.base;
+    emits->push_back(m);
+  };
+  if (op == BROTLI_OPERATION_PROCESS) {
+    while (c.end - c.flushed >= 2 * kStreamPieceBytes) emit(false, c.flushed + kStreamPieceBytes);  // keep one piece back for FINISH
+  } else if (op == BROTLI_OPERATION_FLUSH) {
+    if (c.flushed < c.end) emit(false, c.end);
+  } else if (op == BROTLI_OPERATION_FINISH && !c.finished) {
+    emit(true, c.end);
+    c.finished = 1;
+  }
+  *next = c;
+}
+
 struct BrotliEncoderStateStruct {
   EncoderParams params;
   B200Encoder* enc = nullptr;
   brotli_alloc_func alloc_func = nullptr;  // compressor.rs:60-100: kept for BrotliEncoderMalloc* / Free*
   brotli_free_func free_func = nullptr;
   void* opaque = nullptr;
-  std::vector<uint8_t> input;   // stream bytes [base, base + input.size())
-  uint64_t base = 0;            // absolute stream offset of input[0] (multiple of 4096)
-  uint64_t flushed = 0;         // absolute offset up to which the stream has been turned into output
-  uint64_t dict_len = 0;        // custom dictionary bytes in front of the stream (they count as positions, encode.rs:1247)
+  std::vector<uint8_t> input;   // stream bytes [c.base, c.end)
+  B200StreamCounters c{};       // offsets are absolute; the custom dictionary counts as positions (encode.rs:1247)
   std::vector<uint8_t> output;  // produced, not yet taken
   size_t out_pos = 0;
   uint64_t total_out = 0;       // bytes handed to the caller so far (total_out_, encode.rs:181)
-  bool started = false, finished = false, header_written = false;
+  bool started = false;
 };
 
 struct BrotliEncoderWorkPoolStruct {
@@ -299,18 +360,14 @@ BROTLI_BOOL BrotliEncoderSetParameter(BrotliEncoderState* s, BrotliEncoderParame
   if (!s || s->started) return BROTLI_FALSE;  // encode.rs:289-295
   return apply_param(s->params, (int)p, value) ? BROTLI_TRUE : BROTLI_FALSE;
 }
-// compressor.rs:162 / encode.rs:1205-1260: the last min(size, 2^lgwin - 16) dictionary bytes become window content in
-// front of the stream (they occupy positions), the static dictionary is switched off.  Ignored once input was consumed.
+// compressor.rs:162 / encode.rs:1205-1260: the dictionary rule of stream_start, the static dictionary is switched off.
+// Ignored once input was consumed.
 void BrotliEncoderSetCustomDictionary(BrotliEncoderState* s, size_t size, const uint8_t* dict) {
-  if (!s || s->started || s->dict_len != 0) return;
+  if (!s || s->started || s->c.dict_len != 0) return;
   s->params.no_dictionary = 1;
   if (size <= 1 || !dict) return;
-  const int lw = s->params.lgwin < 10 ? 10 : (s->params.lgwin > 24 ? 24 : s->params.lgwin);
-  const size_t max_dict = ((size_t)1 << lw) - 16;
-  if (size > max_dict) { dict += size - max_dict; size = max_dict; }
-  s->input.assign(dict, dict + size);
-  s->dict_len = size;
-  s->flushed = size;
+  const uint64_t from = stream_start(s->params, size, &s->c);
+  s->input.assign(dict + from, dict + size);
 }
 uint8_t* BrotliEncoderMallocU8(BrotliEncoderState* s, size_t size) {  // compressor.rs:359-371
   if (s && s->alloc_func) return (uint8_t*)s->alloc_func(s->opaque, size);
@@ -331,41 +388,28 @@ void BrotliEncoderFreeUsize(BrotliEncoderState* s, size_t* data, size_t size) { 
   else free(data);
 }
 
-// Compresses the stream bytes [flushed, upto) and appends the result to the output queue.
-static bool state_emit(BrotliEncoderStateStruct* s, bool last, uint64_t upto) {
-  const uint64_t start = s->flushed, len = upto - start;
-  const bool first = !s->header_written;
-  EncoderParams fp = s->params;
-  sanitize_framing(fp);
-  if (len == 0 && !(framed(fp) && first)) {
-    if (last) {
-      if (first) s->output.push_back(6);        // empty stream, encode.rs:1463
-      else if (!fp.bare_stream) s->output.push_back(3);  // ISLAST + ISLASTEMPTY after a byte-aligned flush
-      s->header_written = true;
-    }
+// Runs one emit of stream_plan and appends its output to the output queue.
+static bool state_emit(BrotliEncoderStateStruct* s, const B200StreamEmit& m) {
+  if (m.byte >= 0) {
+    s->output.push_back((uint8_t)m.byte);
+    s->c.header_written = 1;
     return true;
   }
+  const uint64_t len = m.upto - m.start;
   size_t cap = b200_max_compressed_size(len) + 64, got = 0;
   size_t old = s->output.size();
   s->output.resize(old + cap);
-  uint64_t hint = s->params.size_hint ? s->params.size_hint : s->base + s->input.size() - s->dict_len;
   // positions are relative to `base`: once a prefix has been dropped at least a full window precedes `start`, so the
   // window limit min(position, 2^lgwin - 16) is the same in both coordinate systems
-  bool ok = compress_framed(s->enc, s->params, hint, s->input.data(), (size_t)(start - s->base), (size_t)(upto - s->base), first, last,
-                            true, s->output.data() + old, cap, &got);
+  bool ok = compress_framed(s->enc, s->params, m.size_hint, s->input.data(), (size_t)(m.start - m.base), (size_t)(m.upto - m.base),
+                            m.first != 0, m.last != 0, true, s->output.data() + old, cap, &got);
   if (!ok) { s->output.resize(old); return false; }
   s->output.resize(old + got);
-  s->flushed = upto;
-  s->header_written = true;
-  // keep only the match window in front of the unflushed part
-  int lw = s->params.lgwin < 10 ? 10 : (s->params.lgwin > 24 ? 24 : s->params.lgwin);
-  const uint64_t window = ((uint64_t)1 << lw) + 65536;
-  if (s->flushed > s->base + window) {
-    const uint64_t keep_from = (s->flushed - window) & ~(uint64_t)4095;
-    if (keep_from > s->base) {
-      s->input.erase(s->input.begin(), s->input.begin() + (size_t)(keep_from - s->base));
-      s->base = keep_from;
-    }
+  s->c.flushed = m.upto;
+  s->c.header_written = 1;
+  if (m.base_after > s->c.base) {  // keep only the match window in front of the unflushed part
+    s->input.erase(s->input.begin(), s->input.begin() + (size_t)(m.base_after - s->c.base));
+    s->c.base = m.base_after;
   }
   return true;
 }
@@ -375,25 +419,22 @@ BROTLI_BOOL BrotliEncoderCompressStream(BrotliEncoderState* s, BrotliEncoderOper
   if (!s || !available_in || !available_out) return BROTLI_FALSE;
   if (op == BROTLI_OPERATION_EMIT_METADATA) return BROTLI_FALSE;  // not on this path
   DeviceGuard dg;
-  if (*available_in) {
-    if (s->finished || !next_in || !*next_in) return BROTLI_FALSE;
+  const size_t n = *available_in;
+  if (n) {
+    if (s->c.finished || !next_in || !*next_in) return BROTLI_FALSE;
     s->started = true;
-    s->input.insert(s->input.end(), *next_in, *next_in + *available_in);
-    *next_in += *available_in;
+    s->input.insert(s->input.end(), *next_in, *next_in + n);
+    *next_in += n;
     *available_in = 0;
   }
-  const uint64_t end = s->base + s->input.size();
-  while (op == BROTLI_OPERATION_PROCESS && end - s->flushed >= 2 * kStreamPieceBytes) {  // keep one piece back for FINISH
-    if (!state_emit(s, false, s->flushed + kStreamPieceBytes)) return BROTLI_FALSE;
-  }
-  if (op == BROTLI_OPERATION_FLUSH && s->flushed < end) {
-    s->started = true;
-    if (!state_emit(s, false, end)) return BROTLI_FALSE;
-  } else if (op == BROTLI_OPERATION_FINISH && !s->finished) {
-    s->started = true;
-    if (!state_emit(s, true, end)) return BROTLI_FALSE;
-    s->finished = true;
-  }
+  std::vector<B200StreamEmit> plan;
+  B200StreamCounters next;
+  stream_plan(s->params, s->c, (int)op, n, &plan, &next);
+  if ((op == BROTLI_OPERATION_FLUSH && s->c.flushed < next.end) || (op == BROTLI_OPERATION_FINISH && !s->c.finished)) s->started = true;
+  s->c.end = next.end;
+  for (const B200StreamEmit& m : plan)
+    if (!state_emit(s, m)) return BROTLI_FALSE;
+  s->c.finished = next.finished;
   size_t avail = s->output.size() - s->out_pos;
   if (avail && *available_out && next_out && *next_out) {
     size_t n = std::min(avail, *available_out);
@@ -412,7 +453,7 @@ BROTLI_BOOL BrotliEncoderCompressStreaming(BrotliEncoderState* s, BrotliEncoderO
                                            const uint8_t* input_buf, size_t* available_out, uint8_t* output_buf) {
   return BrotliEncoderCompressStream(s, op, available_in, &input_buf, available_out, &output_buf, nullptr);
 }
-BROTLI_BOOL BrotliEncoderIsFinished(BrotliEncoderState* s) { return (s && s->finished && s->out_pos == s->output.size()) ? 1 : 0; }
+BROTLI_BOOL BrotliEncoderIsFinished(BrotliEncoderState* s) { return (s && s->c.finished && s->out_pos == s->output.size()) ? 1 : 0; }
 BROTLI_BOOL BrotliEncoderHasMoreOutput(BrotliEncoderState* s) { return (s && s->out_pos < s->output.size()) ? 1 : 0; }
 const uint8_t* BrotliEncoderTakeOutput(BrotliEncoderState* s, size_t* size) {  // encode.rs:3006-3027
   if (!s || !size) return nullptr;
@@ -622,6 +663,348 @@ int32_t BrotliEncoderCompressWorkPool(BrotliEncoderWorkPool* pool, size_t num_pa
   DeviceGuard dg;
   return compress_multi_impl(pool->encoders, pool->mus, num_params, keys, values, input_size, input, encoded_size, encoded,
                              desired_num_threads);
+}
+
+}  // extern "C"
+
+// ---- device-resident streams (b200_stream_*): stream_plan's emits, compressed and appended on the device ----
+
+// One piece of a device stream onto the caller's output, stream-ordered: out[*cursor, *cursor + size) = src[0, size) and the
+// cursor advances; size is *d_size (src != nullptr), 1 (the single byte `byte`) or 0 (the call only reports the status).  A piece
+// that does not fit in out_cap is not written at all and fails the stream: state[0] = 2, and a failed stream appends nothing more.
+// *status = state[0] afterwards.  Every block reads the cursor before it counts itself done in state[1]; the last block moves the
+// cursor and resets the count.  The copy writes aligned 32-bit words of the output, each put together from two words of the
+// source (4-byte aligned, readable up to size + 8 bytes), and single bytes at the two ends.
+__global__ void __launch_bounds__(256) k_stream_append(const uint8_t* src, const uint64_t* d_size, int byte, uint8_t* out,
+                                                      uint64_t out_cap, uint64_t* cursor, int32_t* status, uint32_t* state) {
+  __shared__ uint64_t s_at, s_n;
+  __shared__ int s_ok;
+  if (threadIdx.x == 0) {
+    s_at = *cursor;
+    s_n = src ? *d_size : (byte >= 0 ? 1 : 0);
+    s_ok = state[0] == 0 && s_at <= out_cap && s_n <= out_cap - s_at;
+  }
+  __syncthreads();
+  const uint64_t at = s_at, n = s_n;
+  if (s_ok && n) {
+    uint8_t* dst = out + at;
+    if (!src) {
+      if (blockIdx.x == 0 && threadIdx.x == 0) dst[0] = (uint8_t)byte;
+    } else {
+      const uint32_t d = (uint32_t)(reinterpret_cast<uintptr_t>(dst) & 3);  // dst[0] is byte d of the first output word
+      uint32_t* dw = reinterpret_cast<uint32_t*>(dst - d);
+      const uint32_t* sw = reinterpret_cast<const uint32_t*>(src);
+      const uint64_t nw = (d + n + 3) >> 2;
+      for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k < nw; k += (uint64_t)gridDim.x * blockDim.x) {
+        // output word k holds source bytes [4k - d, 4k - d + 4): the high bytes of source word k - 1, the low bytes of word k
+        const uint32_t v = __funnelshift_l(k ? sw[k - 1] : 0u, sw[k], 8 * d);
+        const int64_t r = 4 * (int64_t)k - d;
+        if (r >= 0 && r + 4 <= (int64_t)n) {
+          dw[k] = v;
+        } else {
+          for (int j = 0; j < 4; ++j)
+            if (r + j >= 0 && r + j < (int64_t)n) dst[r + j] = (uint8_t)(v >> (8 * j));
+        }
+      }
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    if (atomicAdd(&state[1], 1u) == gridDim.x - 1) {
+      if (s_ok) *cursor = at + n;
+      else if (state[0] == 0) state[0] = 2;
+      state[1] = 0;
+      *status = (int32_t)state[0];
+    }
+  }
+}
+
+struct B200Stream {
+  B200Encoder* enc = nullptr;
+  int device = 0;
+  EncoderParams params;                  // as applied, the custom dictionary's "no static dictionary" included
+  B200StreamCounters c{};
+  uint8_t* win[2] = {nullptr, nullptr};  // window buffers of win_cap bytes; win[cur][0] holds stream byte win_base
+  size_t win_cap = 0;
+  int cur = 0;
+  uint64_t win_base = 0;
+  uint8_t* scratch = nullptr;            // the compressed bytes of one piece
+  size_t scratch_cap = 0;
+  uint64_t* d_word = nullptr;            // [0] the piece's size; [1] k_stream_append's state: failed, blocks done (2 x u32)
+  cudaStream_t last = nullptr;           // the CUDA stream of the last call: b200_stream_destroy frees there
+  cudaEvent_t ev_done = nullptr;         // the end of the last call
+  bool failed = false;                   // a device failure inside a call: later calls are refused
+};
+
+namespace {
+
+bool on_gpu(const void* p, int device) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();
+    return false;
+  }
+  return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == device;
+}
+
+bool stream_capturing(cudaStream_t st) {  // true also when the status cannot be read: the call is then refused
+  cudaStreamCaptureStatus cs;
+  if (cudaStreamIsCapturing(st, &cs) != cudaSuccess) {
+    cudaGetLastError();
+    return true;
+  }
+  return cs != cudaStreamCaptureStatusNone;
+}
+
+// Output bound and largest span piece of one emit: the pieces of compress_span (at most kSpanPiece bytes each), each with the
+// slack b200_encoder_compress_framed_async asks for, plus a prologue and a trailer byte.
+size_t emit_bound(const B200StreamEmit& m, size_t* max_piece) {
+  if (m.byte >= 0) return 1;
+  const uint64_t len = m.upto - m.start;
+  size_t bound = 0;
+  for (uint64_t s = 0; s < len || s == 0; s += kSpanPiece) {
+    const size_t piece = (size_t)std::min<uint64_t>(len - s, kSpanPiece);
+    *max_piece = std::max(*max_piece, piece);
+    bound += b200_max_compressed_size(piece) + 64 + sizeof(B200Prologue::bytes) + 1;
+    if (len == 0) break;
+  }
+  return bound;
+}
+
+// Makes room for n more bytes behind the stream's end.  The kept bytes [base, end) move to the front through the other buffer
+// (a copy between two distinct buffers: overlapping copies are undefined), or into a larger one.  All stream-ordered on st.
+bool stream_room(B200Stream* s, uint64_t n, cudaStream_t st) {
+  if (s->c.end + n - s->win_base <= s->win_cap) return true;
+  const uint64_t live = s->c.end - s->c.base, want = live + n;
+  const uint8_t* from = s->win[s->cur] + (s->c.base - s->win_base);
+  if (want > s->win_cap) {
+    const size_t cap = (size_t)(want + std::max<uint64_t>(want / 2, (uint64_t)1 << 20));
+    void* p = nullptr;
+    if (cudaMallocAsync(&p, cap, st) != cudaSuccess) return false;
+    if (live && cudaMemcpyAsync(p, from, live, cudaMemcpyDeviceToDevice, st) != cudaSuccess) return false;
+    for (uint8_t*& w : s->win) {
+      if (w) cudaFreeAsync(w, st);
+      w = nullptr;
+    }
+    s->win[0] = static_cast<uint8_t*>(p);
+    s->cur = 0;
+    s->win_cap = cap;
+  } else {
+    const int to = s->cur ^ 1;
+    if (!s->win[to] && cudaMallocAsync((void**)&s->win[to], s->win_cap, st) != cudaSuccess) return false;
+    if (live && cudaMemcpyAsync(s->win[to], from, live, cudaMemcpyDeviceToDevice, st) != cudaSuccess) return false;
+    s->cur = to;
+  }
+  s->win_base = s->c.base;
+  return true;
+}
+
+bool stream_append(B200Stream* s, const uint8_t* src, int byte, size_t bound, uint8_t* out, size_t out_cap, uint64_t* cursor,
+                   int32_t* status, cudaStream_t st) {
+  const size_t words = bound / 4 + 2;
+  const unsigned blocks = (unsigned)std::min<size_t>(std::max<size_t>(1, (words + 255) / 256), 1056);  // 8 per SM at most
+  k_stream_append<<<blocks, 256, 0, st>>>(src, s->d_word, byte, out, out_cap, cursor, status, reinterpret_cast<uint32_t*>(s->d_word + 1));
+  return cudaGetLastError() == cudaSuccess;
+}
+
+// Runs one emit on the device: the bytes of state_emit / compress_framed / compress_span for it, piece by piece into the scratch
+// buffer, each piece appended to the caller's output.
+bool stream_run_emit(B200Stream* S, const B200StreamEmit& m, uint8_t* out, size_t out_cap, uint64_t* cursor, int32_t* status,
+                     cudaStream_t st) {
+  if (m.byte >= 0) return stream_append(S, nullptr, m.byte, 1, out, out_cap, cursor, status, st);
+  EncoderParams p = S->params;
+  sanitize_framing(p);
+  const uint8_t* in = S->win[S->cur] + (m.base - S->win_base);
+  const size_t a = (size_t)(m.start - m.base), b = (size_t)(m.upto - m.base);
+  const int lw = p.lgwin < 10 ? 10 : (p.lgwin > 24 ? 24 : p.lgwin);
+  const size_t window = ((size_t)1 << lw) + 65536;
+  const int ctx = p.disable_ctx ? 0 : 1, dict = p.no_dictionary ? 0 : 1;
+  B200Prologue pro;
+  memset(&pro, 0, sizeof(pro));
+  bool has_pro = false, dev_first = m.first != 0, dev_last = m.last != 0, dev_align = true;
+  int trailer = -1;
+  size_t body_a = a;
+  if (framed(p)) {  // compress_framed
+    if (m.first && (p.magic_number || p.catable || a == b)) {
+      dev_first = false;
+      has_pro = true;
+      HostBits w{pro.bytes, sizeof(pro.bytes)};
+      size_t data_off = 0, n2 = 0;
+      write_prologue(w, p, b - a, nullptr, &data_off, &n2);
+      pro.data_off = (uint32_t)data_off;
+      pro.n2 = (uint32_t)n2;
+      body_a += n2;
+      if (body_a == b) write_empty_trailer(w, p, m.last != 0, true);
+      if (!w.ok || (w.pos & 7)) return false;
+      pro.len = (uint32_t)(w.pos >> 3);
+      if (body_a == b) {  // prologue and trailer are the whole emit
+        pro.complete = 1;
+        return b200_encoder_compress_framed_async(S->enc, p.quality, p.lgwin, m.size_hint, ctx, dict, in, b, b, 0, 0, 0, 0, &pro, -1,
+                                                  S->scratch, S->scratch_cap, S->d_word, st) &&
+               stream_append(S, S->scratch, -1, pro.len, out, out_cap, cursor, status, st);
+      }
+    }
+    dev_last = m.last && !p.byte_align && !p.bare_stream;  // the device writes the plain trailer itself
+    dev_align = m.last ? p.byte_align != 0 : true;
+    if (m.last && p.byte_align && !p.bare_stream) trailer = 3;  // ISLAST + ISLASTEMPTY on a byte boundary
+  }
+  for (size_t s = body_a;;) {  // compress_span
+    const size_t e = std::min(b, s + kSpanPiece);
+    const size_t rb = s > window ? ((s - window) & ~(size_t)4095) : 0;
+    const bool f = dev_first && s == body_a, l = e == b;
+    if (!b200_encoder_compress_framed_async(S->enc, p.quality, p.lgwin, m.size_hint, ctx, dict, in + rb, e - rb, s - rb, e - s, f ? 1 : 0,
+                                            (dev_last && l) ? 1 : 0, (l ? (dev_align && !dev_last) : true) ? 1 : 0,
+                                            (has_pro && s == body_a) ? &pro : nullptr, l ? trailer : -1, S->scratch, S->scratch_cap,
+                                            S->d_word, st))
+      return false;
+    if (!stream_append(S, S->scratch, -1, b200_max_compressed_size(e - s) + 64 + sizeof(pro.bytes) + 1, out, out_cap, cursor, status,
+                       st))
+      return false;
+    if (l) return true;
+    s = e;
+  }
+}
+
+bool valid_op(int op) {
+  return op == BROTLI_OPERATION_PROCESS || op == BROTLI_OPERATION_FLUSH || op == BROTLI_OPERATION_FINISH;
+}
+
+bool parse_params(EncoderParams* p, size_t num_params, const BrotliEncoderParameter* keys, const uint32_t* values) {
+  if (num_params && (!keys || !values)) return false;
+  for (size_t i = 0; i < num_params; ++i)
+    if (!apply_param(*p, (int)keys[i], values[i])) return false;
+  return true;
+}
+
+}  // namespace
+
+extern "C" {
+
+B200Stream* b200_stream_create(B200Encoder* e, size_t num_params, const BrotliEncoderParameter* keys, const uint32_t* values,
+                               const uint8_t* d_dict, size_t dict_len, void* stream) {
+  EncoderParams p;
+  if (!e || (dict_len && !d_dict) || !parse_params(&p, num_params, keys, values)) return nullptr;
+  DeviceGuard dg;
+  const int device = b200_encoder_device(e);
+  if (cudaSetDevice(device) != cudaSuccess) return nullptr;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (stream_capturing(st)) return nullptr;
+  if (dict_len > 1 && !on_gpu(d_dict, device)) return nullptr;
+  B200Stream* S = new (std::nothrow) B200Stream();
+  if (!S) return nullptr;
+  S->enc = e;
+  S->device = device;
+  S->last = st;
+  uint64_t from = 0;
+  if (d_dict) {  // BrotliEncoderSetCustomDictionary
+    p.no_dictionary = 1;
+    from = stream_start(p, dict_len, &S->c);
+  }
+  S->params = p;
+  const uint64_t keep = S->c.end;
+  S->c.end = 0;  // the window starts empty and receives the dictionary
+  bool ok = cudaEventCreateWithFlags(&S->ev_done, cudaEventDisableTiming) == cudaSuccess &&
+            cudaMallocAsync((void**)&S->d_word, 16, st) == cudaSuccess && cudaMemsetAsync(S->d_word, 0, 16, st) == cudaSuccess &&
+            stream_room(S, keep, st);
+  if (ok && keep) ok = cudaMemcpyAsync(S->win[S->cur], d_dict + from, keep, cudaMemcpyDeviceToDevice, st) == cudaSuccess;
+  S->c.end = keep;
+  if (ok) ok = cudaEventRecord(S->ev_done, st) == cudaSuccess;
+  if (!ok) {
+    cudaGetLastError();
+    b200_stream_destroy(S);
+    return nullptr;
+  }
+  return S;
+}
+
+size_t b200_stream_output_bound(const B200Stream* S, BrotliEncoderOperation op, size_t n) {
+  if (!S || S->failed || S->c.finished || !valid_op(op)) return 0;
+  std::vector<B200StreamEmit> plan;
+  B200StreamCounters next;
+  stream_plan(S->params, S->c, (int)op, n, &plan, &next);
+  size_t bound = 0, max_piece = 0;
+  for (const B200StreamEmit& m : plan) bound += emit_bound(m, &max_piece);
+  return bound;
+}
+
+int b200_stream_compress_async(B200Stream* S, BrotliEncoderOperation op, const uint8_t* d_in, size_t n, uint8_t* out, size_t out_cap,
+                               uint64_t* d_out_size, int32_t* d_status, void* stream) {
+  if (!S || S->failed || S->c.finished || !valid_op(op) || !out || !d_out_size || !d_status || (n && !d_in)) return 0;
+  DeviceGuard dg;
+  if (cudaSetDevice(S->device) != cudaSuccess) return 0;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (stream_capturing(st)) return 0;
+  // (the pointer queries run in relaxed capture mode: under a global-mode capture on another stream they are no reason to fail)
+  cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+  if (cudaThreadExchangeStreamCaptureMode(&mode) != cudaSuccess) return 0;
+  const bool placed = on_gpu(out, S->device) && on_gpu(d_out_size, S->device) && on_gpu(d_status, S->device) &&
+                      (!n || on_gpu(d_in, S->device));
+  cudaThreadExchangeStreamCaptureMode(&mode);
+  if (!placed) return 0;
+  std::vector<B200StreamEmit> plan;
+  B200StreamCounters next;
+  stream_plan(S->params, S->c, (int)op, n, &plan, &next);
+  size_t max_piece = 0;
+  for (const B200StreamEmit& m : plan) emit_bound(m, &max_piece);
+  S->last = st;
+  bool ok = cudaStreamWaitEvent(st, S->ev_done, 0) == cudaSuccess && stream_room(S, n, st);
+  const size_t need = (b200_max_compressed_size(max_piece) + 128 + 15) & ~(size_t)15;
+  if (ok && !plan.empty() && need > S->scratch_cap) {  // the old scratch is freed behind the work that reads it
+    void* p = nullptr;
+    ok = cudaMallocAsync(&p, need, st) == cudaSuccess;
+    if (ok) {
+      if (S->scratch) cudaFreeAsync(S->scratch, st);
+      S->scratch = static_cast<uint8_t*>(p);
+      S->scratch_cap = need;
+    }
+  }
+  if (ok && n) ok = cudaMemcpyAsync(S->win[S->cur] + (S->c.end - S->win_base), d_in, n, cudaMemcpyDeviceToDevice, st) == cudaSuccess;
+  for (size_t i = 0; ok && i < plan.size(); ++i) ok = stream_run_emit(S, plan[i], out, out_cap, d_out_size, d_status, st);
+  if (ok && plan.empty()) ok = stream_append(S, nullptr, -1, 0, out, out_cap, d_out_size, d_status, st);
+  if (!ok) {  // part of the call may be enqueued: fail the stream on the device too, so that its status reads 2
+    cudaGetLastError();
+    S->failed = true;
+    cudaMemsetAsync(S->d_word + 1, 2, 1, st);
+    stream_append(S, nullptr, -1, 0, out, out_cap, d_out_size, d_status, st);
+    cudaGetLastError();
+    return 0;
+  }
+  S->c = next;
+  cudaEventRecord(S->ev_done, st);
+  return 1;
+}
+
+void b200_stream_destroy(B200Stream* S) {
+  if (!S) return;
+  DeviceGuard dg;
+  cudaSetDevice(S->device);
+  for (void* p : {(void*)S->win[0], (void*)S->win[1], (void*)S->scratch, (void*)S->d_word})
+    if (p) cudaFreeAsync(p, S->last);
+  if (S->ev_done) cudaEventDestroy(S->ev_done);
+  cudaGetLastError();
+  delete S;
+}
+
+int b200_stage_stream_start(size_t num_params, const BrotliEncoderParameter* keys, const uint32_t* values, uint64_t dict_size,
+                            B200StreamCounters* c, uint64_t* dict_from) {
+  EncoderParams p;
+  if (!c || !parse_params(&p, num_params, keys, values)) return 0;
+  const uint64_t from = stream_start(p, dict_size, c);
+  if (dict_from) *dict_from = from;
+  return 1;
+}
+
+int b200_stage_stream_plan(size_t num_params, const BrotliEncoderParameter* keys, const uint32_t* values, const B200StreamCounters* c,
+                           int op, uint64_t n, B200StreamEmit* emits, size_t max_emits, size_t* num_emits, B200StreamCounters* next) {
+  EncoderParams p;
+  if (!c || !next || !num_emits || !valid_op(op) || (n && c->finished) || !parse_params(&p, num_params, keys, values)) return 0;
+  std::vector<B200StreamEmit> plan;
+  stream_plan(p, *c, op, n, &plan, next);
+  if (plan.size() > max_emits || (plan.size() && !emits)) return 0;
+  std::copy(plan.begin(), plan.end(), emits);
+  *num_emits = plan.size();
+  return 1;
 }
 
 }  // extern "C"

@@ -769,14 +769,15 @@ size_t b200_max_compressed_size(size_t n) { return n + (n >> 10) * 8 + 4096; }
 // Pipeline: the input is staged chunk by chunk on a copy stream and chunks alternate between the compute lanes.
 // pro (device input only): the prologue of a framed stream goes in front, and the first chunk starts behind it.
 static bool enqueue_range(B200Encoder* e, const CallPlan& c, const uint8_t* in, cudaMemcpyKind in_kind, uint8_t* out, bool first,
-                          bool last, bool byte_align, std::vector<cudaEvent_t>* h_done, const B200Prologue* pro = nullptr) {
+                          bool last, bool byte_align, std::vector<cudaEvent_t>* h_done, const B200Prologue* pro = nullptr,
+                          const uint8_t* pro_in = nullptr) {
   const size_t nchunks = c.chunks.size();
   e->data_base = c.base;
   uint8_t* dd = e->d_data.as<uint8_t>();
   CUDA_OK(cudaMemsetAsync(out, 0, c.need, e->s_in));
   CUDA_OK(cudaMemsetAsync(e->d_total.p, 0, 8, e->s_in));
   if (pro) {
-    k_prologue<<<1, 32, 0, e->s_in>>>(*pro, in, out, e->d_total.as<uint64_t>(), nullptr);
+    k_prologue<<<1, 32, 0, e->s_in>>>(*pro, pro_in, out, e->d_total.as<uint64_t>(), nullptr);
     e->launches += 1;
   }
   CUDA_OK(cudaMemsetAsync(dd + c.staged, 0, kPad, e->s_in));
@@ -859,14 +860,14 @@ static bool compress_range_impl(B200Encoder* e, int quality, int lgwin, uint64_t
 // more launch on `st`.  Inside a capture it neither waits for nor records ev_call: a graph may not depend on work outside it.
 static bool enqueue_async(B200Encoder* e, const CallPlan& c, const uint8_t* in, bool first, bool last, bool byte_align,
                           bool empty_stream, uint8_t* out, uint64_t* out_size, cudaStream_t st, bool capturing,
-                          const B200Prologue* pro = nullptr, int trailer = -1) {
+                          const B200Prologue* pro = nullptr, int trailer = -1, const uint8_t* pro_in = nullptr) {
   const size_t nchunks = c.chunks.size();
   cudaEvent_t fork = e->sync_events.get(false);
   CUDA_OK(cudaEventRecord(fork, st));
   CUDA_OK(cudaStreamWaitEvent(e->s_in, fork, 0));
   if (!capturing) CUDA_OK(cudaStreamWaitEvent(e->s_in, e->ev_call, 0));
   if (nchunks) {
-    if (!enqueue_range(e, c, in, cudaMemcpyDeviceToDevice, out, first, last, byte_align, nullptr, pro)) return false;
+    if (!enqueue_range(e, c, in, cudaMemcpyDeviceToDevice, out, first, last, byte_align, nullptr, pro, pro_in)) return false;
   } else {
     CUDA_OK(cudaMemsetAsync(out, 0, c.need, e->s_in));
   }
@@ -920,7 +921,8 @@ static int compress_async_impl(B200Encoder* e, int quality, int lgwin, uint64_t 
                                const B200Prologue* pro, int trailer, uint8_t* out, size_t out_cap, uint64_t* out_size, void* stream) {
   if (!e || !e->ok || !out || !out_size) return 0;
   if (n >= 0xFFFFF000ull || range_start > n || range_len > n - range_start) return 0;  // 32-bit positions
-  if (pro && (pro->len > sizeof(pro->bytes) || pro->data_off + pro->n2 > pro->len || pro->n2 > n)) return 0;
+  if (pro && (pro->len > sizeof(pro->bytes) || pro->data_off + pro->n2 > pro->len || pro->n2 > range_start)) return 0;
+  const uint8_t* pro_in = pro ? in + range_start - pro->n2 : nullptr;  // the prologue's data bytes precede the range
   if (cudaSetDevice(e->device) != cudaSuccess) return 0;
   if (out_cap < b200_max_compressed_size(range_len) + 64 || (reinterpret_cast<uintptr_t>(out) & 3)) return 0;
   const bool reads_in = range_len || (pro && pro->n2);
@@ -939,7 +941,7 @@ static int compress_async_impl(B200Encoder* e, int quality, int lgwin, uint64_t 
   if (cs == cudaStreamCaptureStatusInvalidated) return 0;
   const bool capturing = cs == cudaStreamCaptureStatusActive;
   if (pro && pro->complete) {  // the whole stream is prologue and trailer: nothing of the encoder is used
-    k_prologue<<<1, 32, 0, st>>>(*pro, in, out, nullptr, out_size);
+    k_prologue<<<1, 32, 0, st>>>(*pro, pro_in, out, nullptr, out_size);
     return cudaGetLastError() == cudaSuccess ? 1 : 0;
   }
   const int saved_ctx = e->ctx_model, saved_dict = e->use_dict;
@@ -961,7 +963,7 @@ static int compress_async_impl(B200Encoder* e, int quality, int lgwin, uint64_t 
   const bool timing = e->timing;
   e->timing = false;  // stage timing would read events back on the host
   const bool ok = enqueue_async(e, c, in, first != 0, last != 0, byte_align != 0, first && last && n == 0, out, out_size, st,
-                                capturing, pro, trailer);
+                                capturing, pro, trailer, pro_in);
   e->timing = timing;
   if (!ok) {
     if (!capturing) cudaDeviceSynchronize();  // leave no work in flight behind a failed call

@@ -34,7 +34,8 @@ typedef struct B200Prologue {
   uint32_t len, data_off, n2, complete;
 } B200Prologue;
 /* b200_encoder_compress_range_async behind a prologue: the range's first metablock starts at byte pro->len (pro may be NULL), and
- * trailer >= 0 appends that byte behind the range's byte-aligned end.  ctx_model / use_dict apply to this call only. */
+ * trailer >= 0 appends that byte behind the range's byte-aligned end.  The prologue's n2 data bytes are the input bytes right in
+ * front of range_start.  ctx_model / use_dict apply to this call only. */
 int b200_encoder_compress_framed_async(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, int ctx_model, int use_dict,
                                        const uint8_t* in, size_t n, size_t range_start, size_t range_len, int first, int last,
                                        int byte_align, const B200Prologue* pro, int trailer, uint8_t* out, size_t out_cap,

@@ -15,6 +15,10 @@ pub struct BrotliEncoderWorkPool {
 pub struct B200Encoder {
     _private: [u8; 0],
 }
+#[repr(C)]
+pub struct B200Stream {
+    _private: [u8; 0],
+}
 
 pub type brotli_alloc_func = Option<unsafe extern "C" fn(opaque: *mut c_void, size: usize) -> *mut c_void>;
 pub type brotli_free_func = Option<unsafe extern "C" fn(opaque: *mut c_void, address: *mut c_void)>;
@@ -99,6 +103,16 @@ extern "C" {
     pub fn b200_encoder_compress_params_async(e: *mut B200Encoder, num_params: usize, keys: *const u32, values: *const u32,
                                               input: *const u8, n: usize, out: *mut u8, out_cap: usize, out_size: *mut u64,
                                               stream: *mut c_void) -> i32;
+    /// Device-resident stream (include/brotli_b200.h): `d_dict` is a device pointer (null: no custom dictionary); `stream` is a
+    /// `cudaStream_t`.  Null on a refused parameter or dictionary.
+    pub fn b200_stream_create(e: *mut B200Encoder, num_params: usize, keys: *const u32, values: *const u32, d_dict: *const u8,
+                              dict_len: usize, stream: *mut c_void) -> *mut B200Stream;
+    /// One PROCESS / FLUSH / FINISH step (`op` as BrotliEncoderOperation); `input`, `out`, `out_size` and `status` are device
+    /// pointers.  Returns 1 when enqueued.
+    pub fn b200_stream_compress_async(s: *mut B200Stream, op: i32, input: *const u8, n: usize, out: *mut u8, out_cap: usize,
+                                      out_size: *mut u64, status: *mut i32, stream: *mut c_void) -> i32;
+    pub fn b200_stream_output_bound(s: *const B200Stream, op: i32, n: usize) -> usize;
+    pub fn b200_stream_destroy(s: *mut B200Stream);
     pub fn b200_concat_workspace_size(count: u32) -> usize;
     /// Every pointer is a device pointer; `stream` is a `cudaStream_t`.
     pub fn b200_concat_async(streams: *const *const u8, sizes: *const u64, count: u32, window_size: i32, out: *mut u8,
