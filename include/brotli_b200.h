@@ -291,6 +291,11 @@ int b200_concat_async(const uint8_t* const* d_streams, const uint64_t* d_sizes, 
  * kernels; search = 1: the on-demand search at every position (returns 0 where that path does not run: depth < 64, two batches) */
 int b200_stage_match(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n, size_t range_start,
                      size_t range_len, int search, uint32_t* best_out);
+/* stage hook after b200_stage_match with search = 0 at bucket depth 16 / 32 (q5, q6), where best[] is stored through a staging
+ * region cut into slabs of 2^21 positions of each sort batch's payload.  For the range's last batch, cursors[s] = records the
+ * match kernel claimed in slab s and sizes[s] = records slab s must receive (s < cap).  Returns the number of slabs, 0 when
+ * the last call did not stage best[]. */
+int b200_stage_match_slabs(B200Encoder* e, uint32_t* cursors, uint32_t* sizes, uint32_t cap);
 /* stage hook of quality 10 / 11 (n <= one chunk): matches per position hqn[n], hqm[n][16][2] (distance, length word); per parse
  * unit ncmd, tail, ncopy as units[3][nu]; raw commands raw[nu][unit / 2 + 1][3].  b200_hq_unit gives the unit for size_hint n. */
 int b200_stage_hq(B200Encoder* e, int quality, int lgwin, const uint8_t* in, size_t n, uint8_t* hqn, uint32_t* hqm, uint32_t* units,

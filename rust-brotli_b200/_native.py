@@ -59,6 +59,8 @@ def lib():
         L.b200_encoder_last_timings.argtypes = [vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_uint32)]
         L.b200_stage_match.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.c_uint64, vp, sz, sz, sz, ctypes.c_int, vp]
         L.b200_stage_match.restype = ctypes.c_int
+        L.b200_stage_match_slabs.argtypes = [vp, vp, vp, ctypes.c_uint32]
+        L.b200_stage_match_slabs.restype = ctypes.c_int
         L.b200_stage_hq.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp, sz, vp, vp, vp, vp]
         L.b200_stage_hq.restype = ctypes.c_int
         L.b200_hq_unit.argtypes = [vp, ctypes.c_int, ctypes.c_uint64]
@@ -198,6 +200,17 @@ class DeviceEncoder:
         if not ok:
             raise RuntimeError("b200_stage_match failed")
         return out
+
+    def stage_match_slabs(self):
+        """After stage_match (up-front kernels): (cursors, sizes) of the range's last sort batch, uint32 arrays with one entry
+        per best[] slab -- the records the match kernel claimed in each slab and the records each slab must receive."""
+        import numpy as np
+        cursors = np.zeros(64, dtype=np.uint32)
+        sizes = np.zeros(64, dtype=np.uint32)
+        ns = self._L.b200_stage_match_slabs(self._h, cursors.ctypes.data, sizes.ctypes.data, 64)
+        if ns <= 0 or ns > 64:
+            raise RuntimeError("b200_stage_match_slabs failed")
+        return cursors[:ns], sizes[:ns]
 
     def stage_hq(self, data: bytes, quality: int, lgwin: int):
         """Quality 10 / 11 stage results of one chunk: (hqn[n] u8, hqm[n][16][2] u32 (dist, lc), units[3][nu] u32 (ncmd, tail,

@@ -66,6 +66,7 @@ constexpr uint32_t kChunk = BRO_CHUNK_BYTES;   // bytes per pipeline pass (one s
 constexpr uint32_t kBatchMax = 1u << 25;       // positions per sort batch (25-bit packed positions)
 constexpr uint32_t kLookahead = 4096;          // input bytes past a chunk's end that must be resident before it runs
 constexpr int kMaxLanes = 6;
+static_assert((kBatchMax >> BEST_SLAB_BITS) <= BEST_MAX_SLABS, "a batch has more best[] slabs than cursors");
 
 struct EventPool {
   std::vector<cudaEvent_t> ev;
@@ -97,6 +98,8 @@ struct Lane {
   cudaStream_t stream = nullptr;
   DevBuf arena;     // every region of the chunk workspace (layout_chunk)
   Workspace W{};    // the last chunk's workspace: the stage hooks read their results through it
+  const uint32_t* slab_cursor = nullptr;  // the last chunk's last sort batch, when its best[] went through match_store:
+  uint32_t slab_payload = 0;              //   its slab cursors and payload size (b200_stage_match_slabs)
   EventPool marks;  // timing marks: (event, stage that starts there); -1 ends the last stage
   std::vector<int> mark_stage;
   void release() {
@@ -182,6 +185,7 @@ void layout_hq_split(Carve& a, const EncParams& P, const Workspace& W, BsWs* B, 
 
 struct ChunkBufs {  // the regions of a chunk that Workspace does not point to
   SortBufs sort;
+  uint2* stage;         // bucket depth 16 / 32: best[] records of a sort batch, slab-major (match_store)
   ZopfliArgs za;        // quality >= 10
   BsWs bs;              // quality >= 10 with hq_split
   CmWs cm;              //   "
@@ -211,6 +215,7 @@ void layout_chunk(Carve& a, uint32_t c, const EncParams& P, Workspace* W, ChunkB
   W->long_cap = mb_span / LONG_INS + 1;
   if (!hq) {
     W->best = a.take<uint32_t>((size_t)c + 64);
+    if (P.depth <= 32) X->stage = a.take<uint2>(c);  // a batch's payload is at most the chunk
   } else {
     W->hqm = a.take<HqMatch>(((size_t)c + 64) * HQ_MAXM);
     W->hqn = a.take<uint8_t>((size_t)c + 64);
@@ -586,6 +591,7 @@ struct B200Encoder {
     const bool od = od_shape && (ondemand > 1 || (ondemand == 1 && P.depth >= 128 && range_len >= ((uint32_t)4 << 20)));
     DeepArgs da;
     memset(&da, 0, sizeof(da));
+    L.slab_cursor = nullptr;
     for (uint64_t b0 = range_start; b0 < (uint64_t)range_start + range_len; b0 += payload_max) {
       const uint32_t b1 = (uint32_t)std::min<uint64_t>((uint64_t)range_start + range_len, b0 + payload_max);
       uint32_t origin = b0 > window ? (uint32_t)b0 - window : 0u;
@@ -609,6 +615,7 @@ struct B200Encoder {
       ma.max_backward = P.max_backward;
       ma.dict = W.dict;
       ma.use_dict = P.use_dict;
+      const BestStage bs{X.stage, X.sort.state + SORT_ST_SLAB};  // cursors zeroed by run_sort
       const size_t smem = (size_t)(MATCH_THREADS + P.depth) * 6 * 4;
       mark(L, B200_ST_MATCH);
       const uint32_t mgrid = (count + MATCH_THREADS - 1) / MATCH_THREADS;
@@ -640,18 +647,26 @@ struct B200Encoder {
           k_match_level<HQ_LEVEL_DEPTH><<<mgrid, MATCH_THREADS, (size_t)(MATCH_THREADS + HQ_LEVEL_DEPTH) * 3 * 4, stream>>>(aa);
           launches += 1;
         }
-      } else
-      switch (P.depth) {  // bucket depth = 1 << block_bits: 16 (q5) .. 256 (q9, and lgwin <= 16)
-        case 16:
-          k_match_shallow<16><<<mgrid, MATCH_THREADS, smem, stream>>>(ma);
-          break;
-        case 32:
-          k_match_shallow<32><<<mgrid, MATCH_THREADS, smem, stream>>>(ma);
-          break;
-        case 64: k_match_deep<64><<<mgrid, MATCH_THREADS, smem, stream>>>(ma); break;
-        case 128: k_match_deep<128><<<mgrid, MATCH_THREADS, smem, stream>>>(ma); break;
-        case 256: k_match_deep<256><<<mgrid, MATCH_THREADS, smem, stream>>>(ma); break;
-        default: fprintf(stderr, "[brotli_b200] unsupported bucket depth %d\n", P.depth); return false;
+      } else {
+        switch (P.depth) {  // bucket depth = 1 << block_bits: 16 (q5) .. 256 (q9, and lgwin <= 16)
+          case 16:
+            k_match_shallow<16><<<mgrid, MATCH_THREADS, smem, stream>>>(ma, bs);
+            break;
+          case 32:
+            k_match_shallow<32><<<mgrid, MATCH_THREADS, smem, stream>>>(ma, bs);
+            break;
+          case 64: k_match_deep<64><<<mgrid, MATCH_THREADS, smem, stream>>>(ma); break;
+          case 128: k_match_deep<128><<<mgrid, MATCH_THREADS, smem, stream>>>(ma); break;
+          case 256: k_match_deep<256><<<mgrid, MATCH_THREADS, smem, stream>>>(ma); break;
+          default: fprintf(stderr, "[brotli_b200] unsupported bucket depth %d\n", P.depth); return false;
+        }
+        if (P.depth <= 32) {  // k_match_shallow left one record per payload position in X.stage
+          const uint32_t payload = b1 - (uint32_t)b0;
+          k_best_place<<<(payload + 255) / 256, 256, 0, stream>>>(X.stage, payload, ma.best);
+          L.slab_cursor = bs.slab_cursor;
+          L.slab_payload = payload;
+          launches += 1;
+        }
       }
       launches += 1;
     }
@@ -1057,6 +1072,20 @@ int b200_stage_match(B200Encoder* e, int quality, int lgwin, uint64_t size_hint,
   }
   const void* src = search ? e->d_probe.p : (const void*)e->lanes[0].W.best;
   return cudaMemcpy(best_out, src, range_len * 4, cudaMemcpyDeviceToHost) == cudaSuccess;
+}
+
+// test hook: after b200_stage_match with the up-front kernels, the slab cursors of the range's last sort batch (records that
+// match_store claimed in each slab) into cursors[] and the number of records each slab must receive into sizes[], at most cap
+// of each.  Returns the number of slabs, 0 when the last call did not store through match_store.
+int b200_stage_match_slabs(B200Encoder* e, uint32_t* cursors, uint32_t* sizes, uint32_t cap) {
+  if (!e || !e->ok || cudaSetDevice(e->device) != cudaSuccess) return 0;
+  const Lane& L = e->lanes[0];
+  if (!L.slab_cursor) return 0;
+  const uint32_t ns = (L.slab_payload + (1u << BEST_SLAB_BITS) - 1) >> BEST_SLAB_BITS;
+  const uint32_t k = std::min(ns, cap);
+  if (cudaMemcpy(cursors, L.slab_cursor, (size_t)k * 4, cudaMemcpyDeviceToHost) != cudaSuccess) return 0;
+  for (uint32_t s = 0; s < k; ++s) sizes[s] = std::min(1u << BEST_SLAB_BITS, L.slab_payload - (s << BEST_SLAB_BITS));
+  return (int)ns;
 }
 
 // test hook (quality >= 10): matches per position, per-unit results and raw commands of an n-byte buffer (n <= one chunk)

@@ -206,6 +206,7 @@ __device__ __forceinline__ void tma_stage_tile(void* smem_dst, const void* gmem_
 #define SORT_ST_BASE 512    // [2][256] first output index of each digit
 #define SORT_ST_DONE 1024   // k_sort_count CTAs that have added their counts
 #define SORT_ST_TILE 1025   // [2] next tile index of each pass
+#define SORT_ST_SLAB 1032   // [BEST_MAX_SLABS] records claimed in each best[] slab by k_match_shallow in the batch (match_store)
 #define SORT_ST_FLAGS 1056  // [2][num_tiles][256] look-back words: flag bits | count
 #define SORT_LB_AGG (1u << 30)  // count of the digit in this tile alone
 #define SORT_LB_INC (2u << 30)  // count of the digit in this tile and every tile before it
@@ -489,6 +490,50 @@ struct MatchArgs {
   int use_dict;
 };
 
+// best[] of a batch at depth 16 / 32 is written in two steps.  k_match_shallow's positions are in bucket order, so a direct best[p] store puts 4
+// bytes at a random address of the whole payload: every store is a partial 32-byte sector of its own, written back (and
+// fill-read) alone.  Instead the payload [b0, b1) is cut into slabs of 2^BEST_SLAB_BITS positions counted from b0.  Every
+// payload position yields exactly one record, so slab s receives exactly min(2^BEST_SLAB_BITS, b1 - b0 - (s << BEST_SLAB_BITS))
+// records and owns that many 8-byte slots of `stage` from s << BEST_SLAB_BITS on.  match_store bins a CTA's records by slab,
+// claims one contiguous run per slab with one atomic and writes the run; k_best_place then walks `stage` in order, so the live
+// best[] store window is about one slab (8 MB), whose sectors are complete in L2 before they are evicted.  The values placed are
+// the ones a direct store writes; only the order of the records within a slab varies from run to run.
+#define BEST_SLAB_BITS 21
+#define BEST_MAX_SLABS 16  // kBatchMax >> BEST_SLAB_BITS
+static_assert(SORT_ST_SLAB + BEST_MAX_SLABS <= SORT_ST_FLAGS, "slab cursors overlap the look-back words");
+struct BestStage {
+  uint2* stage;           // [payload] (position, value) records, slab-major
+  uint32_t* slab_cursor;  // [BEST_MAX_SLABS] records claimed per slab, zeroed with the sort state
+};
+
+// Called by every thread of the CTA (it synchronises the CTA); `active` threads store best[p] = v of payload position p.
+__device__ __forceinline__ void match_store(const MatchArgs& a, const BestStage& st, bool active, uint32_t p, uint32_t v) {
+  static_assert(MATCH_THREADS >= BEST_MAX_SLABS, "one thread per slab claims the runs");
+  __shared__ uint32_t s_cnt[BEST_MAX_SLABS], s_run[BEST_MAX_SLABS];
+  const uint32_t tid = threadIdx.x, lane = tid & 31u;
+  if (tid < BEST_MAX_SLABS) s_cnt[tid] = 0;
+  __syncthreads();
+  const uint32_t slab = active ? (p - (a.origin + a.payload_begin)) >> BEST_SLAB_BITS : BEST_MAX_SLABS;
+  // lanes of one slab take consecutive ranks of the CTA's run with one shared atomic per warp and slab
+  const uint32_t peers = __match_any_sync(0xffffffffu, slab);
+  const uint32_t leader = (uint32_t)__ffs((int)peers) - 1u;
+  uint32_t first = 0;
+  if (active && lane == leader) first = atomicAdd(&s_cnt[slab], (uint32_t)__popc(peers));
+  const uint32_t rank = __shfl_sync(0xffffffffu, first, leader) + (uint32_t)__popc(peers & ((1u << lane) - 1u));
+  __syncthreads();
+  if (tid < BEST_MAX_SLABS && s_cnt[tid]) s_run[tid] = atomicAdd(&st.slab_cursor[tid], s_cnt[tid]);
+  __syncthreads();
+  if (active) st.stage[((size_t)slab << BEST_SLAB_BITS) + s_run[slab] + rank] = make_uint2(p, v);
+}
+
+// best[pos] = value for the `count` records of `stage`, in order (slab after slab)
+__global__ void __launch_bounds__(256) k_best_place(const uint2* __restrict__ stage, uint32_t count, uint32_t* __restrict__ best) {
+  const uint32_t k = blockIdx.x * 256u + threadIdx.x;
+  if (k >= count) return;
+  const uint2 r = __ldcs(&stage[k]);  // read once
+  best[r.x] = r.y;
+}
+
 // dict_candidate() of bro_dict.cuh with the position's first 16 bytes already in registers and 8-byte word compares
 __device__ __forceinline__ uint32_t dict_candidate_dev(const DictView& D, int hash_type, uint32_t m0, uint32_t m1, uint32_t m2,
                                                        uint32_t m3, const uint8_t* cur, uint32_t max_len, uint32_t mb) {
@@ -553,7 +598,7 @@ __device__ __forceinline__ void match_stage_positions(const MatchArgs& a, int64_
 // comes from one XOR of the second data word), and only candidates that agree on all 8 bytes go through the exact
 // (divergent) evaluation.  Result identical to the sequential newest-first walk: highest score, nearest on ties.
 template <int DEPTH>
-__global__ void __launch_bounds__(MATCH_THREADS) k_match_shallow(MatchArgs a) {
+__global__ void __launch_bounds__(MATCH_THREADS) k_match_shallow(MatchArgs a, BestStage st) {
   extern __shared__ __align__(16) uint32_t smem[];
   constexpr uint32_t E = MATCH_THREADS + (uint32_t)DEPTH;
   uint32_t* s_pos = smem;
@@ -577,11 +622,11 @@ __global__ void __launch_bounds__(MATCH_THREADS) k_match_shallow(MatchArgs a) {
   __syncthreads();
   const uint32_t i = threadIdx.x + (uint32_t)DEPTH;
   const uint32_t prel = s_pos[i];
-  if (prel == 0xFFFFFFFFu || prel < a.payload_begin) return;
-  const uint32_t p = a.origin + prel;
+  const bool active = !(prel == 0xFFFFFFFFu || prel < a.payload_begin);  // inactive threads only take part in match_store
+  const uint32_t p = a.origin + (active ? prel : 0u);
   const uint32_t maxl = bmin(a.lcap, a.n - p);
   uint32_t best_score = BRO_MIN_SCORE, best_len = 0, best_dist = 0;
-  if (a.n - p >= 8) {  // keys of the last 7 positions would depend on bytes past the range: they get no bucket match
+  if (active && a.n - p >= 8) {  // keys of the last 7 positions would depend on bytes past the range: they get no bucket match
     const uint32_t key = s_key[i];
     const uint32_t max_backward = bmin(p, a.max_backward);
     const uint32_t m0 = s_d0[i], m1 = s_d1[i], m2 = s_d2[i], m3 = s_d3[i];
@@ -635,9 +680,9 @@ __global__ void __launch_bounds__(MATCH_THREADS) k_match_shallow(MatchArgs a) {
     }
   }
   uint32_t outv = best_len ? ((best_dist << 8) | best_len) : 0u;
-  if (best_len == 0 && a.use_dict && a.n - p >= 8)  // nothing in the bucket: static dictionary (mod.rs:1797, :1942)
+  if (active && best_len == 0 && a.use_dict && a.n - p >= 8)  // nothing in the bucket: static dictionary (mod.rs:1797, :1942)
     outv = dict_candidate_dev(a.dict, a.hash_type, s_d0[i], s_d1[i], s_d2[i], s_d3[i], a.data + p, a.n - p, bmin(p, a.max_backward));
-  __stcs(&a.best[p], outv);  // scattered, written once, read much later by the parse: do not let it displace the input in L2
+  match_store(a, st, active, p, outv);
 }
 
 // Deep buckets (depth 64..256: q7..q9 and lgwin <= 16).  With one position per lane the survivors of the 4-byte filter are
@@ -786,7 +831,7 @@ __global__ void __launch_bounds__(MATCH_THREADS) k_match_deep(MatchArgs a) {
     } else if (a.use_dict && a.n - p >= 8) {
       r = dict_candidate_dev(a.dict, a.hash_type, s_d0[i], s_d1[i], s_d2[i], s_d3[i], a.data + p, a.n - p, bmin(p, a.max_backward));
     }
-    a.best[p] = r;
+    a.best[p] = r;  // (a long kernel: the scattered store drains under its work, where staging it costs more than it saves)
   }
 }
 
