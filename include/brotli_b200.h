@@ -267,6 +267,22 @@ int b200_stage_stream_start(size_t num_params, const BrotliEncoderParameter* key
                             B200StreamCounters* c, uint64_t* dict_from);
 int b200_stage_stream_plan(size_t num_params, const BrotliEncoderParameter* keys, const uint32_t* values, const B200StreamCounters* c,
                            int op, uint64_t n, B200StreamEmit* emits, size_t max_emits, size_t* num_emits, B200StreamCounters* next);
+/* One device call of the framing rule: compress input bytes [start, end), handed over from `rebase` on (the bytes in front of
+ * start are its window), with the stream header (first), the end of the stream (last) or a byte-aligned end (byte_align). */
+typedef struct B200FramedCall {
+  uint64_t rebase, start, end;
+  int32_t first, last, byte_align;
+} B200FramedCall;
+/* stage hook of the framing rule that BrotliEncoderCompress / CompressStream / CompressMulti, b200_encoder_compress_params_async
+ * and b200_stream_* share (host code, no device needed): how input bytes [a, b) become output, given whether they begin the
+ * stream (first), end it (last) and, when not last, end byte aligned (align_end).  The output is the prologue, the output of each
+ * call in order, then the byte *trailer (-1: none).  prologue (32 bytes) receives the prologue's bytes; prologue_info = {length
+ * in bytes, or -1 when there is none; offset and count of its placeholder bytes, which are input bytes a, a + 1; 1 when the
+ * prologue, its trailing bits included, is the whole output: the one call then compresses nothing}.  Returns 0 for a refused
+ * parameter, a framing that cannot end byte aligned, or more than max_calls calls. */
+int b200_stage_framed_plan(size_t num_params, const BrotliEncoderParameter* keys, const uint32_t* values, uint64_t a, uint64_t b,
+                           int first, int last, int align_end, uint8_t* prologue, int32_t* prologue_info, B200FramedCall* calls,
+                           size_t max_calls, size_t* num_calls, int32_t* trailer);
 
 /* ---- device splice of catable streams (the reference's BroCatli, src/concat/mod.rs; host ABI in broccoli.h) ---- */
 /* Bytes of device workspace b200_concat_async needs for `count` streams. */

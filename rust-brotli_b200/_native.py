@@ -28,6 +28,12 @@ class StreamEmit(ctypes.Structure):
                 ("size_hint", ctypes.c_uint64), ("first", ctypes.c_int32), ("last", ctypes.c_int32), ("byte", ctypes.c_int32)]
 
 
+class FramedCall(ctypes.Structure):
+    """B200FramedCall (include/brotli_b200.h): one device call of the framing rule."""
+    _fields_ = [("rebase", ctypes.c_uint64), ("start", ctypes.c_uint64), ("end", ctypes.c_uint64), ("first", ctypes.c_int32),
+                ("last", ctypes.c_int32), ("byte_align", ctypes.c_int32)]
+
+
 def lib():
     global _lib
     if _lib is None:
@@ -81,6 +87,9 @@ def lib():
         L.b200_stage_stream_plan.argtypes = [sz, vp, vp, P(StreamCounters), ctypes.c_int, ctypes.c_uint64, P(StreamEmit), sz, P(sz),
                                              P(StreamCounters)]
         L.b200_stage_stream_plan.restype = ctypes.c_int
+        L.b200_stage_framed_plan.argtypes = [sz, vp, vp, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_int, ctypes.c_int, ctypes.c_int, vp,
+                                             P(ctypes.c_int32), P(FramedCall), sz, P(sz), P(ctypes.c_int32)]
+        L.b200_stage_framed_plan.restype = ctypes.c_int
         _lib = L
     return _lib
 
@@ -270,3 +279,19 @@ def stream_plan(key_values, counters: StreamCounters, op: int, n: int, max_emits
                                         op, n, emits, max_emits, ctypes.byref(count), ctypes.byref(nxt)):
         return None
     return list(emits[:count.value]), nxt
+
+
+def framed_plan(key_values, a: int, b: int, first: bool, last: bool, align_end: bool, max_calls: int = 16):
+    """b200_stage_framed_plan: (prologue, calls, trailer) of input bytes [a, b), or None when the plan is refused.  prologue is
+    None or (bytes, data_off, n2, complete); calls are (rebase, start, end, first, last, byte_align) tuples; trailer is -1 or
+    the byte behind the last call."""
+    k, keys, vals = key_value_arrays(key_values)
+    pro, info = (ctypes.c_uint8 * 32)(), (ctypes.c_int32 * 4)()
+    calls, count, trailer = (FramedCall * max_calls)(), ctypes.c_size_t(0), ctypes.c_int32(0)
+    if not lib().b200_stage_framed_plan(k, ctypes.cast(keys, ctypes.c_void_p), ctypes.cast(vals, ctypes.c_void_p), a, b, int(first),
+                                        int(last), int(align_end), pro, info, calls, max_calls, ctypes.byref(count),
+                                        ctypes.byref(trailer)):
+        return None
+    prologue = None if info[0] < 0 else (bytes(pro[:info[0]]), info[1], info[2], bool(info[3]))
+    return prologue, [(c.rebase, c.start, c.end, bool(c.first), bool(c.last), bool(c.byte_align)) for c in calls[:count.value]], \
+        trailer.value

@@ -37,6 +37,11 @@ void sanitize_framing(EncoderParams& p) {
 }
 bool framed(const EncoderParams& p) { return p.catable || p.appendable || p.magic_number || p.byte_align || p.bare_stream; }
 
+// lgwin as the stream runs it: the window bits, the custom dictionary's share and the rebase window all use this value.
+int window_bits(const EncoderParams& p) { return p.lgwin < 10 ? 10 : (p.lgwin > 24 ? 24 : p.lgwin); }
+// The bytes kept in front of a position when input is handed over from a later base: the window and 64 KiB.
+uint64_t rebase_window(const EncoderParams& p) { return ((uint64_t)1 << window_bits(p)) + 65536; }
+
 // Applies one parameter; a value this path cannot honour leaves `p` unchanged and returns false (the reference's
 // set_parameter returns false only after initialisation, encode.rs:289-295 -- here "accepted" also means "will act").
 bool apply_param(EncoderParams& p, int key, uint32_t value) {
@@ -63,6 +68,13 @@ bool apply_param(EncoderParams& p, int key, uint32_t value) {
       if (!(key >= 150 && key <= 173)) return false;
   }
   p = q;
+  return true;
+}
+
+bool parse_params(EncoderParams* p, size_t num_params, const BrotliEncoderParameter* keys, const uint32_t* values) {
+  if (num_params && (!keys || !values)) return false;
+  for (size_t i = 0; i < num_params; ++i)
+    if (!apply_param(*p, (int)keys[i], values[i])) return false;
   return true;
 }
 
@@ -108,8 +120,7 @@ constexpr size_t kStreamPieceBytes = (size_t)4 * BRO_CHUNK_BYTES_CAPI;
 static uint64_t stream_start(const EncoderParams& p, uint64_t size, B200StreamCounters* c) {
   memset(c, 0, sizeof(*c));
   if (size <= 1) return size;
-  const int lw = p.lgwin < 10 ? 10 : (p.lgwin > 24 ? 24 : p.lgwin);
-  const uint64_t keep = std::min<uint64_t>(size, ((uint64_t)1 << lw) - 16);
+  const uint64_t keep = std::min<uint64_t>(size, ((uint64_t)1 << window_bits(p)) - 16);
   c->dict_len = c->flushed = c->end = keep;
   return size - keep;
 }
@@ -123,8 +134,7 @@ static void stream_plan(const EncoderParams& p, const B200StreamCounters& c0, in
   sanitize_framing(fp);
   B200StreamCounters c = c0;
   c.end += n;
-  const int lw = p.lgwin < 10 ? 10 : (p.lgwin > 24 ? 24 : p.lgwin);
-  const uint64_t window = ((uint64_t)1 << lw) + 65536;
+  const uint64_t window = rebase_window(p);
   const uint64_t hint = p.size_hint ? p.size_hint : c.end - c.dict_len;  // the input so far
   auto emit = [&](bool last, uint64_t upto) {
     B200StreamEmit m;
@@ -183,36 +193,7 @@ struct BrotliEncoderWorkPoolStruct {
   std::vector<std::mutex*> mus;        // calls that share the pool are serialised per encoder (threading/mod.rs work pool)
 };
 
-// Compresses input[a, b) of an n-byte stream into out (host).  Positions inside the device encoder are 32-bit, so the
-// span is cut into pieces of at most kSpanPiece bytes, each handed over relative to a base at most one window in front of
-// it; pieces in the middle end byte aligned.  first/last: stream header / final empty metablock belong to this span;
-// align_end: a span that is not last ends byte aligned.
-constexpr size_t kSpanPiece = (size_t)1 << 30;
-static bool compress_span(B200Encoder* enc, const EncoderParams& p, uint64_t hint, const uint8_t* input, size_t a, size_t b,
-                          bool first, bool last, bool align_end, uint8_t* out, size_t out_cap, size_t* out_size) {
-  const int lw = p.lgwin < 10 ? 10 : (p.lgwin > 24 ? 24 : p.lgwin);
-  const size_t window = ((size_t)1 << lw) + 65536;
-  size_t off = 0;
-  b200_encoder_set_option(enc, B200_OPT_CTX_MODEL, p.disable_ctx ? 0 : 1);
-  b200_encoder_set_option(enc, B200_OPT_DICT, p.no_dictionary ? 0 : 1);
-  for (size_t s = a; s < b || s == a;) {
-    const size_t e = std::min(b, s + kSpanPiece);
-    // once a full window precedes `s`, min(position, 2^lgwin - 16) is the same in rebased coordinates
-    const size_t rb = s > window ? ((s - window) & ~(size_t)4095) : 0;
-    size_t got = 0;
-    const bool f = first && s == a, l = e == b;
-    if (!b200_encoder_compress_range(enc, p.quality, p.lgwin, hint, input + rb, e - rb, s - rb, e - s, f ? 1 : 0,
-                                     (last && l) ? 1 : 0, (l ? (align_end && !last) : true) ? 1 : 0, out + off, out_cap - off, &got, 0))
-      return false;
-    off += got;
-    if (e == b) break;
-    s = e;
-  }
-  *out_size = off;
-  return true;
-}
-
-// ---- stream framing around compress_span (catable / appendable / magic_number / byte_align / bare_stream) ----
+// ---- stream framing (catable / appendable / magic_number / byte_align / bare_stream) ----
 struct HostBits {  // LSB-first bit writer into a bounded host buffer
   uint8_t* out; size_t cap; uint64_t pos = 0; bool ok = true;
   void put(uint32_t nbits, uint64_t v) {
@@ -233,13 +214,12 @@ static void put_window_bits(HostBits& w, int lgwin) {  // EncodeWindowBits encod
 }
 // The prologue of a framed stream of `len` bytes (p sanitised): [window bits unless catable && bare] [magic-number metadata
 // metablock, brotli_bit_stream.rs:2869-2896] [catable: the first min(2, len) bytes as an uncompressed metablock,
-// encode.rs:2285-2333].  data: those first bytes, or nullptr to leave zeros in their place (the device copies them in);
-// *data_off / *n2: where they are and how many.  Shared by compress_framed and b200_encoder_compress_params_async.
-static void write_prologue(HostBits& w, const EncoderParams& p, size_t len, const uint8_t* data, size_t* data_off, size_t* n2) {
-  const int lw = p.lgwin < 10 ? 10 : (p.lgwin > 24 ? 24 : p.lgwin);
+// encode.rs:2285-2333 -- a stitched stream's literal contexts then never look into the previous file].  Zeros stand in for those
+// bytes; *data_off / *n2: where they are and how many.
+static void write_prologue(HostBits& w, const EncoderParams& p, size_t len, size_t* data_off, size_t* n2) {
   *data_off = 0;
   *n2 = 0;
-  if (!(p.catable && p.bare_stream)) put_window_bits(w, lw);
+  if (!(p.catable && p.bare_stream)) put_window_bits(w, window_bits(p));
   if (p.magic_number) {
     uint8_t sh[10]; size_t nsh = 0;
     for (uint64_t v = p.size_hint;;) {  // encode_base_128 brotli_bit_stream.rs:2855-2867
@@ -259,7 +239,7 @@ static void write_prologue(HostBits& w, const EncoderParams& p, size_t len, cons
     w.align();
     *data_off = (size_t)(w.pos >> 3);
     const uint8_t zeros[2] = {0, 0};
-    w.bytes(data ? data : zeros, *n2);
+    w.bytes(zeros, *n2);
   }
 }
 // The end of a framed stream with nothing (left) to compress behind the prologue (WriteEmptyLastBlocksInternal
@@ -270,48 +250,93 @@ static void write_empty_trailer(HostBits& w, const EncoderParams& p, bool last, 
     if (!p.bare_stream) { w.put(2, 3); w.align(); }
   } else if (align_end && (w.pos & 7)) { w.put(6, 6); w.align(); }
 }
-// Compresses input[a, b) like compress_span and wraps it in the framing `p` asks for:
-//   first: [window bits unless catable && bare] [magic-number metadata metablock, brotli_bit_stream.rs:2869-2896]
-//          [catable: the first min(2, len) bytes as an uncompressed metablock, encode.rs:2285-2333 -- a stitched stream's literal
-//          contexts then never look into the previous file]
-//   last:  [byte_align: padding metablock][unless bare: the empty last metablock]  (WriteEmptyLastBlocksInternal encode.rs:1928-1940)
-// Data metablocks never carry ISLAST on this path, so "appendable" (encode.rs:1973-1975) needs nothing more, and every
-// metablock starts with an unknown distance cache, which is what catable's 0x7ffffff0 cache (encode.rs:693-703) asks for.
-static bool compress_framed(B200Encoder* enc, EncoderParams p, uint64_t hint, const uint8_t* input, size_t a, size_t b, bool first,
-                            bool last, bool align_end, uint8_t* out, size_t out_cap, size_t* out_size) {
+
+// How input bytes [a, b) become output: the prologue, the output of each device call in order, then the trailer byte.  Every
+// entry point executes this plan: compress_framed on the host, b200_encoder_compress_params_async and the device stream.
+struct FramedPlan {
+  bool has_pro = false;
+  B200Prologue pro{};                 // its n2 data bytes are zeros: the executor puts input bytes a, a + 1 there
+  std::vector<B200FramedCall> calls;  // at least one: a complete prologue goes with one call that compresses nothing
+  int trailer = -1;                   // appended behind the last call
+  int ctx_model = 1, use_dict = 1;    // the encoder options of every call (catable switches the static dictionary off)
+};
+
+// first / last: the stream header / its end belong to [a, b); align_end: when not last, the output ends byte aligned.  A framed
+// stream's header is a host-built prologue when it carries more than the window bits, or when there is nothing to compress; the
+// device writes a plain 2-bit ending itself, a byte-aligned one ends with trailer byte 3.  Data metablocks never carry ISLAST on
+// this path, so "appendable" (encode.rs:1973-1975) needs nothing more, and every metablock starts with an unknown distance cache,
+// which is what catable's 0x7ffffff0 cache (encode.rs:693-703) asks for.  Positions inside the device encoder are 32-bit, so the
+// body is cut into calls of at most kSpanPiece bytes, each handed over from a base at most one rebase window in front of it;
+// calls in the middle end byte aligned.  Returns false when the output could not end on a byte boundary.
+constexpr size_t kSpanPiece = (size_t)1 << 30;
+static bool framed_plan(EncoderParams p, uint64_t a, uint64_t b, bool first, bool last, bool align_end, FramedPlan* f) {
   sanitize_framing(p);
-  if (!framed(p)) return compress_span(enc, p, hint, input, a, b, first, last, align_end, out, out_cap, out_size);
-  HostBits w{out, out_cap};
-  size_t body_a = a;
-  bool dev_first = first;
-  if (first && (p.magic_number || p.catable || a == b)) {
-    dev_first = false;
-    size_t data_off, n2;
-    write_prologue(w, p, b - a, input + a, &data_off, &n2);
+  f->ctx_model = p.disable_ctx ? 0 : 1;
+  f->use_dict = p.no_dictionary ? 0 : 1;
+  f->has_pro = framed(p) && ((first && (p.magic_number || p.catable)) || a == b);
+  uint64_t body_a = a;
+  if (f->has_pro) {
+    HostBits w{f->pro.bytes, sizeof(f->pro.bytes)};
+    size_t data_off = 0, n2 = 0;
+    if (first) write_prologue(w, p, b - a, &data_off, &n2);
     body_a += n2;
+    if (body_a == b) write_empty_trailer(w, p, last, align_end);
+    if (!w.ok || (w.pos & 7)) return false;
+    f->pro.len = (uint32_t)(w.pos >> 3);
+    f->pro.data_off = (uint32_t)data_off;
+    f->pro.n2 = (uint32_t)n2;
+    f->pro.complete = body_a == b;
   }
-  if (!w.ok) return false;
-  size_t off = (size_t)(w.pos >> 3);
-  if (body_a < b) {
-    if (w.pos & 7) return false;  // cannot happen: a prologue in front of data ends with a byte-aligned metablock
-    // the device writes the plain 2-bit trailer itself when no alignment is asked for
-    const bool dev_last = last && !p.byte_align && !p.bare_stream;
-    const bool dev_align = last ? (p.byte_align != 0) : align_end;
+  const bool dev_first = first && !f->has_pro, dev_last = last && !p.byte_align && !p.bare_stream;
+  const bool dev_align = last ? p.byte_align != 0 : align_end;
+  if (body_a < b && last && p.byte_align && !p.bare_stream) f->trailer = 3;  // ISLAST + ISLASTEMPTY on a byte boundary
+  const uint64_t window = rebase_window(p);
+  for (uint64_t s = body_a;;) {
+    const uint64_t e = std::min<uint64_t>(b, s + kSpanPiece);
+    const bool l = e == b;
+    // once a full window precedes `s`, min(position, 2^lgwin - 16) is the same in rebased coordinates
+    f->calls.push_back(B200FramedCall{s > window ? ((s - window) & ~(uint64_t)4095) : 0, s, e, dev_first && s == body_a,
+                                      dev_last && l, l ? (dev_align && !dev_last) : true});
+    if (l) return true;
+    s = e;
+  }
+}
+
+// Compresses input[a, b) into out (host): framed_plan's prologue with its data bytes, each call through the blocking device path,
+// then the trailer byte.
+static bool compress_framed(B200Encoder* enc, const EncoderParams& p, uint64_t hint, const uint8_t* input, size_t a, size_t b,
+                            bool first, bool last, bool align_end, uint8_t* out, size_t out_cap, size_t* out_size) {
+  FramedPlan f;
+  if (!framed_plan(p, a, b, first, last, align_end, &f) || f.pro.len > out_cap) return false;
+  std::copy(f.pro.bytes, f.pro.bytes + f.pro.len, out);
+  std::copy(input + a, input + a + f.pro.n2, out + f.pro.data_off);
+  size_t off = f.pro.len;
+  b200_encoder_set_option(enc, B200_OPT_CTX_MODEL, f.ctx_model);
+  b200_encoder_set_option(enc, B200_OPT_DICT, f.use_dict);
+  for (const B200FramedCall& c : f.calls) {
     size_t got = 0;
-    if (!compress_span(enc, p, hint, input, body_a, b, dev_first, dev_last, dev_align, out + off, out_cap - off, &got)) return false;
+    if (!b200_encoder_compress_range(enc, p.quality, p.lgwin, hint, input + c.rebase, c.end - c.rebase, c.start - c.rebase,
+                                     c.end - c.start, c.first, c.last, c.byte_align, out + off, out_cap - off, &got, 0))
+      return false;
     off += got;
-    if (last && p.byte_align && !p.bare_stream) {
-      if (off >= out_cap) return false;
-      out[off++] = 3;  // ISLAST + ISLASTEMPTY on a byte boundary
-    }
-    *out_size = off;
-    return true;
   }
-  // nothing (left) to compress: the trailer follows the prologue directly
-  write_empty_trailer(w, p, last, align_end);
-  if (!w.ok || (w.pos & 7)) return false;
-  *out_size = (size_t)(w.pos >> 3);
+  if (f.trailer >= 0) {
+    if (off >= out_cap) return false;
+    out[off++] = (uint8_t)f.trailer;
+  }
+  *out_size = off;
   return true;
+}
+
+// Enqueues call i of plan f over `in` on the device, stream-ordered: a kernel writes the prologue in front of the first call's
+// output (its data bytes are the input in front of that call's range), and the trailer byte follows the last.
+static int enqueue_framed_call(B200Encoder* e, const EncoderParams& p, uint64_t hint, const FramedPlan& f, size_t i, const uint8_t* in,
+                               uint8_t* out, size_t out_cap, uint64_t* out_size, void* stream) {
+  const B200FramedCall& c = f.calls[i];
+  return b200_encoder_compress_framed_async(e, p.quality, p.lgwin, hint, f.ctx_model, f.use_dict, in + c.rebase, c.end - c.rebase,
+                                            c.start - c.rebase, c.end - c.start, c.first, c.last, c.byte_align,
+                                            (f.has_pro && i == 0) ? &f.pro : nullptr, i + 1 == f.calls.size() ? f.trailer : -1, out,
+                                            out_cap, out_size, stream);
 }
 
 extern "C" {
@@ -484,7 +509,7 @@ BROTLI_BOOL BrotliEncoderCompress(int quality, int lgwin, BrotliEncoderMode mode
     EncoderParams p;
     p.quality = quality;
     p.lgwin = lgwin;
-    ok = compress_span(enc, p, input_size, input, 0, input_size, true, true, false, encoded, out_cap, &got);
+    ok = compress_framed(enc, p, input_size, input, 0, input_size, true, true, false, encoded, out_cap, &got);
   }
   if (!ok) {  // no CPU-produced stream, ever: a device failure (or a too-small output buffer) is reported as failure
     *encoded_size = 0;
@@ -494,46 +519,17 @@ BROTLI_BOOL BrotliEncoderCompress(int quality, int lgwin, BrotliEncoderMode mode
   return BROTLI_TRUE;
 }
 
-// One complete stream of the n device bytes at `in`, stream-ordered on `stream`: the bytes of compress_framed(first, last) --
-// which BrotliEncoderCompressStream with one FINISH runs -- with the prologue written by a kernel and the body compressed behind it.
+// One complete stream of the n device bytes at `in`, stream-ordered on `stream`: framed_plan(0, n, first, last) -- which
+// BrotliEncoderCompressStream with one FINISH runs -- enqueued as its one device call.
 int b200_encoder_compress_params_async(B200Encoder* e, size_t num_params, const BrotliEncoderParameter* keys, const uint32_t* values,
                                        const uint8_t* in, size_t n, uint8_t* out, size_t out_cap, uint64_t* out_size, void* stream) {
-  if (!e || (num_params && (!keys || !values))) return 0;
-  if (n >= kSpanPiece) return 0;  // one span piece: longer inputs are cut into pieces by compress_span
+  if (!e) return 0;
+  if (n >= kSpanPiece) return 0;  // one call: longer inputs are cut into several (a catable body starts two bytes in)
   if (out_cap < b200_max_compressed_size(n) + 64) return 0;
   EncoderParams p;
-  for (size_t i = 0; i < num_params; ++i)
-    if (!apply_param(p, (int)keys[i], values[i])) return 0;
-  sanitize_framing(p);
-  const uint64_t hint = p.size_hint ? p.size_hint : n;
-  const int ctx = p.disable_ctx ? 0 : 1, dict = p.no_dictionary ? 0 : 1;
-  if (!framed(p))
-    return b200_encoder_compress_framed_async(e, p.quality, p.lgwin, hint, ctx, dict, in, n, 0, n, 1, 1, 0, nullptr, -1, out, out_cap,
-                                              out_size, stream);
-  B200Prologue pro;
-  memset(&pro, 0, sizeof(pro));
-  HostBits w{pro.bytes, sizeof(pro.bytes)};
-  size_t body_a = 0, data_off = 0, n2 = 0;
-  const bool has_prologue = p.magic_number || p.catable || n == 0;
-  if (has_prologue) write_prologue(w, p, n, nullptr, &data_off, &n2);
-  body_a = n2;
-  if (!w.ok) return 0;
-  pro.data_off = (uint32_t)data_off;
-  pro.n2 = (uint32_t)n2;
-  if (body_a < n) {  // as compress_framed: the device writes the plain trailer itself unless the stream ends byte aligned
-    if (w.pos & 7) return 0;
-    pro.len = (uint32_t)(w.pos >> 3);
-    const bool dev_last = !p.byte_align && !p.bare_stream;
-    return b200_encoder_compress_framed_async(e, p.quality, p.lgwin, hint, ctx, dict, in, n, body_a, n - body_a, has_prologue ? 0 : 1,
-                                              dev_last ? 1 : 0, p.byte_align ? 1 : 0, has_prologue ? &pro : nullptr,
-                                              (p.byte_align && !p.bare_stream) ? 3 : -1, out, out_cap, out_size, stream);
-  }
-  write_empty_trailer(w, p, true, true);
-  if (!w.ok || (w.pos & 7)) return 0;
-  pro.len = (uint32_t)(w.pos >> 3);
-  pro.complete = 1;
-  return b200_encoder_compress_framed_async(e, p.quality, p.lgwin, hint, ctx, dict, in, n, n, 0, 0, 0, 0, &pro, -1, out, out_cap,
-                                            out_size, stream);
+  FramedPlan f;
+  if (!parse_params(&p, num_params, keys, values) || !framed_plan(p, 0, n, true, true, true, &f)) return 0;
+  return enqueue_framed_call(e, p, p.size_hint ? p.size_hint : n, f, 0, in, out, out_cap, out_size, stream);
 }
 
 // ---- multi ----
@@ -757,17 +753,26 @@ bool stream_capturing(cudaStream_t st) {  // true also when the status cannot be
   return cs != cudaStreamCaptureStatusNone;
 }
 
-// Output bound and largest span piece of one emit: the pieces of compress_span (at most kSpanPiece bytes each), each with the
-// slack b200_encoder_compress_framed_async asks for, plus a prologue and a trailer byte.
-size_t emit_bound(const B200StreamEmit& m, size_t* max_piece) {
+// The framing of one emit of stream_plan: its range of the window buffer, whose first byte is stream offset m.base.
+bool plan_emit(const EncoderParams& p, const B200StreamEmit& m, FramedPlan* f) {
+  return framed_plan(p, m.start - m.base, m.upto - m.base, m.first != 0, m.last != 0, true, f);
+}
+
+// The input bytes the output of call i stands for: its range and, for the first call, the prologue's data bytes.
+size_t call_piece(const FramedPlan& f, size_t i) { return (size_t)(f.calls[i].end - f.calls[i].start) + (i ? 0 : f.pro.n2); }
+
+// Output bound of one call: the slack b200_encoder_compress_framed_async asks for, plus a prologue and a trailer byte.
+size_t piece_bound(size_t piece) { return b200_max_compressed_size(piece) + 64 + sizeof(B200Prologue::bytes) + 1; }
+
+// Output bound and largest piece of one emit.
+size_t emit_bound(const EncoderParams& p, const B200StreamEmit& m, size_t* max_piece) {
   if (m.byte >= 0) return 1;
-  const uint64_t len = m.upto - m.start;
+  FramedPlan f;
+  if (!plan_emit(p, m, &f)) return 0;  // the call then fails before it appends anything
   size_t bound = 0;
-  for (uint64_t s = 0; s < len || s == 0; s += kSpanPiece) {
-    const size_t piece = (size_t)std::min<uint64_t>(len - s, kSpanPiece);
-    *max_piece = std::max(*max_piece, piece);
-    bound += b200_max_compressed_size(piece) + 64 + sizeof(B200Prologue::bytes) + 1;
-    if (len == 0) break;
+  for (size_t i = 0; i < f.calls.size(); ++i) {
+    *max_piece = std::max(*max_piece, call_piece(f, i));
+    bound += piece_bound(call_piece(f, i));
   }
   return bound;
 }
@@ -808,73 +813,22 @@ bool stream_append(B200Stream* s, const uint8_t* src, int byte, size_t bound, ui
   return cudaGetLastError() == cudaSuccess;
 }
 
-// Runs one emit on the device: the bytes of state_emit / compress_framed / compress_span for it, piece by piece into the scratch
-// buffer, each piece appended to the caller's output.
+// Runs one emit on the device: each call of its plan into the scratch buffer, then appended to the caller's output.
 bool stream_run_emit(B200Stream* S, const B200StreamEmit& m, uint8_t* out, size_t out_cap, uint64_t* cursor, int32_t* status,
                      cudaStream_t st) {
   if (m.byte >= 0) return stream_append(S, nullptr, m.byte, 1, out, out_cap, cursor, status, st);
-  EncoderParams p = S->params;
-  sanitize_framing(p);
+  FramedPlan f;
+  if (!plan_emit(S->params, m, &f)) return false;
   const uint8_t* in = S->win[S->cur] + (m.base - S->win_base);
-  const size_t a = (size_t)(m.start - m.base), b = (size_t)(m.upto - m.base);
-  const int lw = p.lgwin < 10 ? 10 : (p.lgwin > 24 ? 24 : p.lgwin);
-  const size_t window = ((size_t)1 << lw) + 65536;
-  const int ctx = p.disable_ctx ? 0 : 1, dict = p.no_dictionary ? 0 : 1;
-  B200Prologue pro;
-  memset(&pro, 0, sizeof(pro));
-  bool has_pro = false, dev_first = m.first != 0, dev_last = m.last != 0, dev_align = true;
-  int trailer = -1;
-  size_t body_a = a;
-  if (framed(p)) {  // compress_framed
-    if (m.first && (p.magic_number || p.catable || a == b)) {
-      dev_first = false;
-      has_pro = true;
-      HostBits w{pro.bytes, sizeof(pro.bytes)};
-      size_t data_off = 0, n2 = 0;
-      write_prologue(w, p, b - a, nullptr, &data_off, &n2);
-      pro.data_off = (uint32_t)data_off;
-      pro.n2 = (uint32_t)n2;
-      body_a += n2;
-      if (body_a == b) write_empty_trailer(w, p, m.last != 0, true);
-      if (!w.ok || (w.pos & 7)) return false;
-      pro.len = (uint32_t)(w.pos >> 3);
-      if (body_a == b) {  // prologue and trailer are the whole emit
-        pro.complete = 1;
-        return b200_encoder_compress_framed_async(S->enc, p.quality, p.lgwin, m.size_hint, ctx, dict, in, b, b, 0, 0, 0, 0, &pro, -1,
-                                                  S->scratch, S->scratch_cap, S->d_word, st) &&
-               stream_append(S, S->scratch, -1, pro.len, out, out_cap, cursor, status, st);
-      }
-    }
-    dev_last = m.last && !p.byte_align && !p.bare_stream;  // the device writes the plain trailer itself
-    dev_align = m.last ? p.byte_align != 0 : true;
-    if (m.last && p.byte_align && !p.bare_stream) trailer = 3;  // ISLAST + ISLASTEMPTY on a byte boundary
-  }
-  for (size_t s = body_a;;) {  // compress_span
-    const size_t e = std::min(b, s + kSpanPiece);
-    const size_t rb = s > window ? ((s - window) & ~(size_t)4095) : 0;
-    const bool f = dev_first && s == body_a, l = e == b;
-    if (!b200_encoder_compress_framed_async(S->enc, p.quality, p.lgwin, m.size_hint, ctx, dict, in + rb, e - rb, s - rb, e - s, f ? 1 : 0,
-                                            (dev_last && l) ? 1 : 0, (l ? (dev_align && !dev_last) : true) ? 1 : 0,
-                                            (has_pro && s == body_a) ? &pro : nullptr, l ? trailer : -1, S->scratch, S->scratch_cap,
-                                            S->d_word, st))
+  for (size_t i = 0; i < f.calls.size(); ++i)
+    if (!enqueue_framed_call(S->enc, S->params, m.size_hint, f, i, in, S->scratch, S->scratch_cap, S->d_word, st) ||
+        !stream_append(S, S->scratch, -1, piece_bound(call_piece(f, i)), out, out_cap, cursor, status, st))
       return false;
-    if (!stream_append(S, S->scratch, -1, b200_max_compressed_size(e - s) + 64 + sizeof(pro.bytes) + 1, out, out_cap, cursor, status,
-                       st))
-      return false;
-    if (l) return true;
-    s = e;
-  }
+  return true;
 }
 
 bool valid_op(int op) {
   return op == BROTLI_OPERATION_PROCESS || op == BROTLI_OPERATION_FLUSH || op == BROTLI_OPERATION_FINISH;
-}
-
-bool parse_params(EncoderParams* p, size_t num_params, const BrotliEncoderParameter* keys, const uint32_t* values) {
-  if (num_params && (!keys || !values)) return false;
-  for (size_t i = 0; i < num_params; ++i)
-    if (!apply_param(*p, (int)keys[i], values[i])) return false;
-  return true;
 }
 
 }  // namespace
@@ -924,7 +878,7 @@ size_t b200_stream_output_bound(const B200Stream* S, BrotliEncoderOperation op, 
   B200StreamCounters next;
   stream_plan(S->params, S->c, (int)op, n, &plan, &next);
   size_t bound = 0, max_piece = 0;
-  for (const B200StreamEmit& m : plan) bound += emit_bound(m, &max_piece);
+  for (const B200StreamEmit& m : plan) bound += emit_bound(S->params, m, &max_piece);
   return bound;
 }
 
@@ -946,7 +900,7 @@ int b200_stream_compress_async(B200Stream* S, BrotliEncoderOperation op, const u
   B200StreamCounters next;
   stream_plan(S->params, S->c, (int)op, n, &plan, &next);
   size_t max_piece = 0;
-  for (const B200StreamEmit& m : plan) emit_bound(m, &max_piece);
+  for (const B200StreamEmit& m : plan) emit_bound(S->params, m, &max_piece);
   S->last = st;
   bool ok = cudaStreamWaitEvent(st, S->ev_done, 0) == cudaSuccess && stream_room(S, n, st);
   const size_t need = (b200_max_compressed_size(max_piece) + 128 + 15) & ~(size_t)15;
@@ -984,6 +938,23 @@ void b200_stream_destroy(B200Stream* S) {
   if (S->ev_done) cudaEventDestroy(S->ev_done);
   cudaGetLastError();
   delete S;
+}
+
+int b200_stage_framed_plan(size_t num_params, const BrotliEncoderParameter* keys, const uint32_t* values, uint64_t a, uint64_t b,
+                           int first, int last, int align_end, uint8_t* prologue, int32_t* prologue_info, B200FramedCall* calls,
+                           size_t max_calls, size_t* num_calls, int32_t* trailer) {
+  EncoderParams p;
+  FramedPlan f;
+  if (!prologue || !prologue_info || !num_calls || !trailer || b < a || !parse_params(&p, num_params, keys, values) ||
+      !framed_plan(p, a, b, first != 0, last != 0, align_end != 0, &f) || f.calls.size() > max_calls || !calls)
+    return 0;
+  memcpy(prologue, f.pro.bytes, sizeof(f.pro.bytes));
+  const int32_t info[4] = {f.has_pro ? (int32_t)f.pro.len : -1, (int32_t)f.pro.data_off, (int32_t)f.pro.n2, (int32_t)f.pro.complete};
+  memcpy(prologue_info, info, sizeof(info));
+  std::copy(f.calls.begin(), f.calls.end(), calls);
+  *num_calls = f.calls.size();
+  *trailer = f.trailer;
+  return 1;
 }
 
 int b200_stage_stream_start(size_t num_params, const BrotliEncoderParameter* keys, const uint32_t* values, uint64_t dict_size,

@@ -461,7 +461,7 @@ def test_compress_multi_across_physical_gpus(encoder):
     parts = []
     for i in range(8):
         a, b = i * len(d) // 8, (i + 1) * len(d) // 8
-        win = (1 << 22) + 65536  # csrc/bro_capi.cu compress_span: the prefix handed over is re-based to one window (+ slack) in front
+        win = (1 << 22) + 65536  # csrc/bro_capi.cu framed_plan: the prefix handed over is re-based to one window (+ slack) in front
         lo = ((a - win) & ~4095) if a > win else 0
         parts.append(encoder.compress_range(d[lo:b], a - lo, b - a, 9, 22, i == 0, i == 7, True, size_hint=b - a))
     assert b"".join(parts) == c
