@@ -85,7 +85,11 @@ BrotliEncoderState* BrotliEncoderCreateInstance(brotli_alloc_func alloc_func, br
  * VERSION, size hint), BYTE_ALIGN (padding metablock in front of the final empty one), BARE_STREAM (no final metablock; with
  * CATABLE no window bits either).  Streams made with CATABLE go through the reference's BroCatli (src/concat/mod.rs).
  * QUALITY: 5..9 run the hash-chain family, 10 and 11 the optimal-parse family; values below 5 run as 5 (the q0..q4
- * hashers are not built) -- b200_effective_quality() reports the quality that will really be used. */
+ * hashers are not built) -- b200_effective_quality() reports the quality that will really be used.
+ * Q9_5 ("quality 9.5", encode.rs:834-893): quality 10 / 11 parse with the hash chains (10: H9; 11: H5 / H6 with 512-deep buckets)
+ * and keep their metablock builder (context mode, block split, clustered context maps, distance parameters); at every quality
+ * it lowers the size hint above which H6 is chosen from 4 MiB to 1 MiB.  The one-shot BrotliEncoderCompress never sets it.
+ * The other research knobs (151..173 apart from the framing keys) are accepted and have no effect. */
 BROTLI_BOOL BrotliEncoderSetParameter(BrotliEncoderState* state, BrotliEncoderParameter p, uint32_t value);
 /* :128 */
 void BrotliEncoderDestroyInstance(BrotliEncoderState* state);

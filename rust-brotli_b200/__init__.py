@@ -21,6 +21,7 @@ from ._native import DeviceEncoder, lib  # noqa: F401
 # BrotliEncoderParameter (src/enc/parameters.rs:1-32)
 BROTLI_PARAM_MODE, BROTLI_PARAM_QUALITY, BROTLI_PARAM_LGWIN, BROTLI_PARAM_LGBLOCK = 0, 1, 2, 3
 BROTLI_PARAM_DISABLE_LITERAL_CONTEXT_MODELING, BROTLI_PARAM_SIZE_HINT, BROTLI_PARAM_LARGE_WINDOW = 4, 5, 6
+BROTLI_PARAM_Q9_5 = 150
 BROTLI_PARAM_CATABLE, BROTLI_PARAM_APPENDABLE, BROTLI_PARAM_MAGIC_NUMBER = 167, 168, 169
 BROTLI_PARAM_NO_DICTIONARY, BROTLI_PARAM_BYTE_ALIGN, BROTLI_PARAM_BARE_STREAM = 170, 172, 173
 BROTLI_OPERATION_PROCESS, BROTLI_OPERATION_FLUSH, BROTLI_OPERATION_FINISH = 0, 1, 2
@@ -54,6 +55,7 @@ class BrotliEncoderParams:
     byte_align: bool = False
     bare_stream: bool = False
     use_dictionary: bool = True
+    q9_5: bool = False  # "quality 9.5": with quality 10 / 11, the hash-chain parse under the quality 10 / 11 metablock builder
 
     def as_key_values(self):
         kv = [(BROTLI_PARAM_QUALITY, self.quality), (BROTLI_PARAM_LGWIN, self.lgwin), (BROTLI_PARAM_MODE, self.mode)]
@@ -65,6 +67,8 @@ class BrotliEncoderParams:
             kv.append((BROTLI_PARAM_LGBLOCK, self.lgblock))
         if not self.use_dictionary:
             kv.append((BROTLI_PARAM_NO_DICTIONARY, 1))
+        if self.q9_5:
+            kv.append((BROTLI_PARAM_Q9_5, 1))
         # framing parameters are forwarded, never dropped: the C ABI refuses the ones this path cannot produce
         for key, on in ((BROTLI_PARAM_CATABLE, self.catable), (BROTLI_PARAM_APPENDABLE, self.appendable),
                         (BROTLI_PARAM_MAGIC_NUMBER, self.magic_number), (BROTLI_PARAM_BYTE_ALIGN, self.byte_align),

@@ -12,6 +12,7 @@ NUM_STAGES = 7
 STAGE_NAMES = ("sort", "match", "parse", "finalize", "split", "header", "emit")
 OPT_CTX_MODEL, OPT_TIMING, OPT_LANES, OPT_DICT = 6, 7, 8, 9
 OPT_HQ_SPLIT, OPT_HQ_UNIT, OPT_ONDEMAND, OPT_HQ_LEVELS = 12, 13, 15, 16
+OPT_Q9_5 = 17
 
 _lib = None
 

@@ -25,6 +25,7 @@ struct EncoderParams {  // the subset of BrotliEncoderParams (backward_reference
   uint64_t size_hint = 0;
   int disable_ctx = 0;
   int no_dictionary = 0;
+  int q9_5 = 0;         // BROTLI_PARAM_Q9_5 (encode.rs:221): quality 10 / 11 parse with the hash chains (bro_hq.cuh: default_enc_params)
   int catable = 0, appendable = 0, magic_number = 0, byte_align = 0, bare_stream = 0;
 };
 
@@ -57,6 +58,7 @@ bool apply_param(EncoderParams& p, int key, uint32_t value) {
     case BROTLI_PARAM_SIZE_HINT: q.size_hint = value; break;
     case BROTLI_PARAM_NO_DICTIONARY: q.no_dictionary = value != 0; break;
     case BROTLI_PARAM_LARGE_WINDOW: if (value != 0) return false; break;  // windows above 2^24 are not produced
+    case BROTLI_PARAM_Q9_5: q.q9_5 = value != 0; break;
     // stream framing (encode.rs:264-283; acted on by compress_framed below)
     case BROTLI_PARAM_CATABLE: q.catable = value != 0; if (!q.appendable) q.appendable = value != 0; break;
     case BROTLI_PARAM_APPENDABLE: q.appendable = value != 0; break;
@@ -65,7 +67,7 @@ bool apply_param(EncoderParams& p, int key, uint32_t value) {
     case BROTLI_PARAM_BARE_STREAM: q.bare_stream = value != 0; if (!q.byte_align) q.byte_align = value != 0; break;
     default:
       // research / divans knobs of the reference (stride, prior, cdf speeds ...) have no effect on this path
-      if (!(key >= 150 && key <= 173)) return false;
+      if (!(key >= 151 && key <= 173)) return false;
   }
   p = q;
   return true;
@@ -259,6 +261,7 @@ struct FramedPlan {
   std::vector<B200FramedCall> calls;  // at least one: a complete prologue goes with one call that compresses nothing
   int trailer = -1;                   // appended behind the last call
   int ctx_model = 1, use_dict = 1;    // the encoder options of every call (catable switches the static dictionary off)
+  int q9_5 = 0;
 };
 
 // first / last: the stream header / its end belong to [a, b); align_end: when not last, the output ends byte aligned.  A framed
@@ -273,6 +276,7 @@ static bool framed_plan(EncoderParams p, uint64_t a, uint64_t b, bool first, boo
   sanitize_framing(p);
   f->ctx_model = p.disable_ctx ? 0 : 1;
   f->use_dict = p.no_dictionary ? 0 : 1;
+  f->q9_5 = p.q9_5;
   f->has_pro = framed(p) && ((first && (p.magic_number || p.catable)) || a == b);
   uint64_t body_a = a;
   if (f->has_pro) {
@@ -313,6 +317,7 @@ static bool compress_framed(B200Encoder* enc, const EncoderParams& p, uint64_t h
   size_t off = f.pro.len;
   b200_encoder_set_option(enc, B200_OPT_CTX_MODEL, f.ctx_model);
   b200_encoder_set_option(enc, B200_OPT_DICT, f.use_dict);
+  b200_encoder_set_option(enc, B200_OPT_Q9_5, f.q9_5);
   for (const B200FramedCall& c : f.calls) {
     size_t got = 0;
     if (!b200_encoder_compress_range(enc, p.quality, p.lgwin, hint, input + c.rebase, c.end - c.rebase, c.start - c.rebase,
@@ -333,7 +338,7 @@ static bool compress_framed(B200Encoder* enc, const EncoderParams& p, uint64_t h
 static int enqueue_framed_call(B200Encoder* e, const EncoderParams& p, uint64_t hint, const FramedPlan& f, size_t i, const uint8_t* in,
                                uint8_t* out, size_t out_cap, uint64_t* out_size, void* stream) {
   const B200FramedCall& c = f.calls[i];
-  return b200_encoder_compress_framed_async(e, p.quality, p.lgwin, hint, f.ctx_model, f.use_dict, in + c.rebase, c.end - c.rebase,
+  return b200_encoder_compress_framed_async(e, p.quality, p.lgwin, hint, f.ctx_model, f.use_dict, f.q9_5, in + c.rebase, c.end - c.rebase,
                                             c.start - c.rebase, c.end - c.start, c.first, c.last, c.byte_align,
                                             (f.has_pro && i == 0) ? &f.pro : nullptr, i + 1 == f.calls.size() ? f.trailer : -1, out,
                                             out_cap, out_size, stream);

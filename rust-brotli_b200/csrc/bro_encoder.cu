@@ -138,7 +138,7 @@ SortBufs layout_sort(Carve& a, uint32_t nb) {
   return s;
 }
 
-// workspaces of the quality >= 10 histogram stage (BrotliSplitBlock + context-map clustering); W's capacities are set
+// workspaces of the quality 10 / 11 histogram stage (BrotliSplitBlock + context-map clustering); W's capacities are set
 void layout_hq_split(Carve& a, const EncParams& P, const Workspace& W, BsWs* B, CmWs* M) {
   const uint32_t NM = W.num_mb;
   const uint32_t mb_span = P.unit * P.mb_units;
@@ -186,8 +186,8 @@ void layout_hq_split(Carve& a, const EncParams& P, const Workspace& W, BsWs* B, 
 struct ChunkBufs {  // the regions of a chunk that Workspace does not point to
   SortBufs sort;
   uint2* stage;         // bucket depth 16 / 32: best[] records of a sort batch, slab-major (match_store)
-  ZopfliArgs za;        // quality >= 10
-  BsWs bs;              // quality >= 10 with hq_split
+  ZopfliArgs za;        // zopfli
+  BsWs bs;              // hq_meta with hq_split
   CmWs cm;              //   "
   uint64_t* dist_cost;  //   "   [num_mb][64] cost of every (NPOSTFIX, NDIRECT)
 };
@@ -199,7 +199,7 @@ void layout_chunk(Carve& a, uint32_t c, const EncParams& P, Workspace* W, ChunkB
   const uint32_t NM = (NU + P.mb_units - 1) / P.mb_units;
   const uint32_t cu = P.unit / 2 + 1;
   const uint32_t cmd_cap = mb_span / 2 + 2;
-  const bool hq = P.quality >= 10, hq_split = hq && P.hq_split;
+  const bool hq = P.zopfli, hq_split = P.hq_meta && P.hq_split;
   W->num_units = NU;
   W->num_mb = NM;
   W->cmd_cap = cmd_cap;
@@ -322,7 +322,8 @@ struct B200Encoder {
   bool ok = false;
   // configuration knobs (tests flip these)
   int ctx_model = 1, use_dict = 1, hq_split = 1, hq_levels = HQ_MAX_LEVELS;
-  uint32_t hq_unit = 0;  // parse unit of the shortest-path parse (quality >= 10); 0 = 8 KiB at q10, 16 KiB at q11 (DESIGN.md)
+  int q9_5 = 0;           // BROTLI_PARAM_Q9_5: quality 10 / 11 parse with the hash chains (default_enc_params)
+  uint32_t hq_unit = 0;  // parse unit of the shortest-path parse (quality 10 / 11); 0 = 8 KiB at q10, 16 KiB at q11 (DESIGN.md)
   int num_lanes = 4;
   int ondemand = 1;       // q7..q9: search deep buckets where the parse stands (1) or for every position up front (0, A/B)
   Lane lanes[kMaxLanes];
@@ -395,11 +396,11 @@ struct B200Encoder {
   }
 
   void fill_params(EncParams* P, int quality, int lgwin, uint64_t size_hint) const {
-    default_enc_params(P, quality, lgwin, size_hint > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)size_hint);
+    default_enc_params(P, quality, lgwin, size_hint > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)size_hint, q9_5);
     P->ctx_model = ctx_model;
     P->use_dict = use_dict;
     P->hq_split = hq_split;
-    if (P->quality >= 10) {
+    if (P->zopfli) {
       P->hq_levels = hq_levels;
       if (hq_unit) {  // same metablock span
         const uint32_t span = P->unit * P->mb_units;
@@ -583,11 +584,11 @@ struct B200Encoder {
     // ---- sort + match, batch by batch ----
     const uint32_t window = 1u << P.lgwin;
     const uint32_t payload_max = kBatchMax - window - 4096;
-    // q7..q9 (bucket depth >= 64): the parse searches the buckets on demand when the chunk is a single sort batch
-    // (depth >= 128 -- q8, q9 and the lgwin <= 16 configurations -- gains most on JSON logs and periodic data, where the walk
+    // q7..q9 and 9.5 (bucket depth >= 64): the parse searches the buckets on demand when the chunk is a single sort batch
+    // (depth >= 128 -- q8, q9, 9.5 and the lgwin <= 16 configurations -- gains most on JSON logs and periodic data, where the walk
     // visits few positions; depth 64 (q7) and inputs of a few units are faster up front.  ondemand = 2 forces the on-demand path
     // for every deep configuration, 0 switches it off.)
-    const bool od_shape = P.quality < 10 && (P.depth == 64 || P.depth == 128 || P.depth == 256) && range_len <= payload_max;
+    const bool od_shape = !P.zopfli && (P.depth == 64 || P.depth == 128 || P.depth == 256 || P.depth == 512) && range_len <= payload_max;
     const bool od = od_shape && (ondemand > 1 || (ondemand == 1 && P.depth >= 128 && range_len >= ((uint32_t)4 << 20)));
     DeepArgs da;
     memset(&da, 0, sizeof(da));
@@ -627,10 +628,11 @@ struct B200Encoder {
           const uint32_t pg = (range_len + 7) / 8;
           if (P.depth == 64) k_od_probe<64><<<pg, 256, 0, stream>>>(da, range_start, range_len, od_probe);
           else if (P.depth == 128) k_od_probe<128><<<pg, 256, 0, stream>>>(da, range_start, range_len, od_probe);
-          else k_od_probe<256><<<pg, 256, 0, stream>>>(da, range_start, range_len, od_probe);
+          else if (P.depth == 256) k_od_probe<256><<<pg, 256, 0, stream>>>(da, range_start, range_len, od_probe);
+          else k_od_probe<512><<<pg, 256, 0, stream>>>(da, range_start, range_len, od_probe);
         }
       } else
-      if (P.quality >= 10) {  // all matches of every position
+      if (P.zopfli) {  // all matches of every position
         MatchAllArgs aa;
         aa.m = ma;
         aa.hqm = W.hqm - (size_t)range_start * HQ_MAXM;
@@ -648,7 +650,7 @@ struct B200Encoder {
           launches += 1;
         }
       } else {
-        switch (P.depth) {  // bucket depth = 1 << block_bits: 16 (q5) .. 256 (q9, and lgwin <= 16)
+        switch (P.depth) {  // bucket depth = 1 << block_bits: 16 (q5) .. 256 (q9, and lgwin <= 16), 512 (quality 11 with Q9_5)
           case 16:
             k_match_shallow<16><<<mgrid, MATCH_THREADS, smem, stream>>>(ma, bs);
             break;
@@ -658,6 +660,7 @@ struct B200Encoder {
           case 64: k_match_deep<64><<<mgrid, MATCH_THREADS, smem, stream>>>(ma); break;
           case 128: k_match_deep<128><<<mgrid, MATCH_THREADS, smem, stream>>>(ma); break;
           case 256: k_match_deep<256><<<mgrid, MATCH_THREADS, smem, stream>>>(ma); break;
+          case 512: k_match_deep<512><<<mgrid, MATCH_THREADS, smem, stream>>>(ma); break;
           default: fprintf(stderr, "[brotli_b200] unsupported bucket depth %d\n", P.depth); return false;
         }
         if (P.depth <= 32) {  // k_match_shallow left one record per payload position in X.stage
@@ -671,13 +674,14 @@ struct B200Encoder {
       launches += 1;
     }
     mark(L, B200_ST_PARSE);
-    if (P.quality >= 10) {  // shortest-path parse, one unit per warp
+    if (P.zopfli) {  // shortest-path parse, one unit per warp
       for (int phase = 1; phase <= (P.quality >= 11 ? 2 : 1); ++phase) k_zopfli<<<W.num_units, 32, 0, stream>>>(W, X.za, phase);
-    } else {  // greedy / lazy parse: fill_params gives n_last 4 at depth 16 / 32 (q5, q6), 10 at 64 / 128 (q7, q8), 16 at 256
+    } else {  // greedy / lazy parse: fill_params gives n_last 4 at depth 16 / 32 (q5, q6), 10 at 64 / 128 (q7, q8), 16 at 256 / 512
       const uint32_t pg = (W.num_units + PARSE_WARPS - 1) / PARSE_WARPS;
       if (od && P.n_last == 10 && P.depth == 64) k_parse_ondemand<10, 64><<<pg, PARSE_WARPS * 32, 0, stream>>>(W, da);
       else if (od && P.n_last == 10 && P.depth == 128) k_parse_ondemand<10, 128><<<pg, PARSE_WARPS * 32, 0, stream>>>(W, da);
       else if (od && P.n_last == 16 && P.depth == 256) k_parse_ondemand<16, 256><<<pg, PARSE_WARPS * 32, 0, stream>>>(W, da);
+      else if (od && P.n_last == 16 && P.depth == 512) k_parse_ondemand<16, 512><<<pg, PARSE_WARPS * 32, 0, stream>>>(W, da);
       else if (!od && P.n_last == 4) k_parse_pair<<<(W.num_units + 4 * PARSE_WARPS - 1) / (4 * PARSE_WARPS), PARSE_WARPS * 32, 0, stream>>>(W);
       else if (!od && P.n_last == 10) k_parse<10><<<pg, PARSE_WARPS * 32, 0, stream>>>(W);
       else if (!od && P.n_last == 16) k_parse<16><<<pg, PARSE_WARPS * 32, 0, stream>>>(W);
@@ -687,7 +691,7 @@ struct B200Encoder {
     k_fin_count<<<W.num_mb, 1024, 0, stream>>>(W);
     k_fin_write<<<(W.num_units + PARSE_WARPS - 1) / PARSE_WARPS, PARSE_WARPS * 32, 0, stream>>>(W);
     k_fin_dist<<<W.num_mb, 1024, 0, stream>>>(W);
-    if (P.quality >= 10 && P.hq_split) {  // NPOSTFIX / NDIRECT of every metablock (metablock.rs:152-207), commands re-coded
+    if (P.hq_meta && P.hq_split) {  // NPOSTFIX / NDIRECT of every metablock (metablock.rs:152-207), commands re-coded
       k_dist_cost<<<dim3(64, W.num_mb), 256, 0, stream>>>(W, X.dist_cost);
       k_dist_apply<<<dim3(64, W.num_mb), 256, 0, stream>>>(W, X.dist_cost);
       launches += 2;
@@ -701,7 +705,7 @@ struct B200Encoder {
     mark(L, B200_ST_SPLIT);
     {
       dim3 g(W.num_mb, 3);
-      if (P.quality >= 10 && P.hq_split) { if (!run_hq_split(stream, W, X.bs, X.cm)) return false; }
+      if (P.hq_meta && P.hq_split) { if (!run_hq_split(stream, W, X.bs, X.cm)) return false; }
       else k_split_greedy<<<g, SPLIT_THREADS, SPLIT_SMEM_WORDS * 4, stream>>>(W);
     }
     mark(L, B200_ST_HEADER);
@@ -770,6 +774,7 @@ int b200_encoder_set_option(B200Encoder* e, int option, uint32_t value) {
     case B200_OPT_HQ_LEVELS: e->hq_levels = value > HQ_MAX_LEVELS ? HQ_MAX_LEVELS : (int)value; return 1;
     case B200_OPT_HQ_SPLIT: e->hq_split = (int)value; return 1;
     case B200_OPT_HQ_UNIT: e->hq_unit = value; return 1;
+    case B200_OPT_Q9_5: e->q9_5 = value != 0; return 1;
     case B200_OPT_LANES: e->num_lanes = value < 1 ? 1 : (value > (uint32_t)kMaxLanes ? kMaxLanes : (int)value); return 1;
   }
   return 0;
@@ -908,20 +913,26 @@ int b200_encoder_reserve(B200Encoder* e, int quality, int lgwin, uint64_t size_h
   // Every call with the same or smaller arguments must fit.  Workspaces grow with the range and the window, but not with the
   // quality or the size hint: smaller parse units (quality 10 against 11, small size hints at 10 / 11) need more per byte.  So
   // each quality family up to `quality` is sized at each size-hint class up to `size_hint`; the staged input is bounded over
-  // every range start.
+  // every range start.  Quality 10 / 11 include their Q9_5 layout (the hash-chain regions next to the histogram-stage ones),
+  // whatever the encoder's B200_OPT_Q9_5 is now, because the framed entry points set it per call.
   const uint64_t hint = size_hint ? size_hint : n;
   const int q_max = effective_quality(quality);
   const uint64_t hints[3] = {hint, std::min<uint64_t>(hint, 1u << 20), std::min<uint64_t>(hint, 256u << 10)};
   CallSizes s;
+  const int saved_q95 = e->q9_5;
   for (int q : {5, 10, 11}) {
     if (q > q_max) break;
-    for (uint64_t h : hints) {
-      if (!h) continue;
-      CallPlan c;
-      e->plan_call(&c, q, lgwin, h, n - range_len, range_len);
-      s.cover(e->sizes_of(c));
+    for (int q95 = 0; q95 <= (q >= 10 ? 1 : 0); ++q95) {
+      e->q9_5 = q95;
+      for (uint64_t h : hints) {
+        if (!h) continue;
+        CallPlan c;
+        e->plan_call(&c, q, lgwin, h, n - range_len, range_len);
+        s.cover(e->sizes_of(c));
+      }
     }
   }
+  e->q9_5 = saved_q95;
   if (range_len) {
     EncParams P;
     e->fill_params(&P, quality, lgwin, hint);
@@ -931,7 +942,7 @@ int b200_encoder_reserve(B200Encoder* e, int quality, int lgwin, uint64_t size_h
 }
 
 // b200_encoder_compress_range_async and, with a prologue / trailer / per-call options, b200_encoder_compress_framed_async
-static int compress_async_impl(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, int ctx_model, int use_dict,
+static int compress_async_impl(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, int ctx_model, int use_dict, int q9_5,
                                const uint8_t* in, size_t n, size_t range_start, size_t range_len, int first, int last, int byte_align,
                                const B200Prologue* pro, int trailer, uint8_t* out, size_t out_cap, uint64_t* out_size, void* stream) {
   if (!e || !e->ok || !out || !out_size) return 0;
@@ -959,13 +970,15 @@ static int compress_async_impl(B200Encoder* e, int quality, int lgwin, uint64_t 
     k_prologue<<<1, 32, 0, st>>>(*pro, pro_in, out, nullptr, out_size);
     return cudaGetLastError() == cudaSuccess ? 1 : 0;
   }
-  const int saved_ctx = e->ctx_model, saved_dict = e->use_dict;
+  const int saved_ctx = e->ctx_model, saved_dict = e->use_dict, saved_q95 = e->q9_5;
   if (ctx_model >= 0) e->ctx_model = ctx_model;  // read into the call's parameters by plan_call, restored below
   if (use_dict >= 0) e->use_dict = use_dict;
+  if (q9_5 >= 0) e->q9_5 = q9_5;
   CallPlan c;
   e->plan_call(&c, quality, lgwin, size_hint ? size_hint : n, range_start, range_len);
   e->ctx_model = saved_ctx;
   e->use_dict = saved_dict;
+  e->q9_5 = saved_q95;
   if (pro && c.chunks.empty()) return 0;  // a prologue in front of nothing is a complete one
   if (!e->provide(e->sizes_of(c), !capturing)) {
     if (capturing) fprintf(stderr, "[brotli_b200] a call inside a CUDA graph capture needs b200_encoder_reserve first\n");
@@ -990,15 +1003,15 @@ static int compress_async_impl(B200Encoder* e, int quality, int lgwin, uint64_t 
 int b200_encoder_compress_range_async(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n,
                                       size_t range_start, size_t range_len, int first, int last, int byte_align, uint8_t* out,
                                       size_t out_cap, uint64_t* out_size, void* stream) {
-  return compress_async_impl(e, quality, lgwin, size_hint, -1, -1, in, n, range_start, range_len, first, last, byte_align, nullptr, -1,
+  return compress_async_impl(e, quality, lgwin, size_hint, -1, -1, -1, in, n, range_start, range_len, first, last, byte_align, nullptr, -1,
                              out, out_cap, out_size, stream);
 }
 
 int b200_encoder_compress_framed_async(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, int ctx_model, int use_dict,
-                                       const uint8_t* in, size_t n, size_t range_start, size_t range_len, int first, int last,
-                                       int byte_align, const B200Prologue* pro, int trailer, uint8_t* out, size_t out_cap,
+                                       int q9_5, const uint8_t* in, size_t n, size_t range_start, size_t range_len, int first,
+                                       int last, int byte_align, const B200Prologue* pro, int trailer, uint8_t* out, size_t out_cap,
                                        uint64_t* out_size, void* stream) {
-  return compress_async_impl(e, quality, lgwin, size_hint, ctx_model, use_dict, in, n, range_start, range_len, first, last, byte_align,
+  return compress_async_impl(e, quality, lgwin, size_hint, ctx_model, use_dict, q9_5, in, n, range_start, range_len, first, last, byte_align,
                              pro, trailer, out, out_cap, out_size, stream);
 }
 
@@ -1040,20 +1053,21 @@ int b200_encoder_last_timings(B200Encoder* e, float* ms, uint32_t* launches) {
   return 1;
 }
 
-// test hook (quality 5..9): best[] of the match stage for the range [range_start, range_start + range_len) of an n-byte buffer
-// (host in, host out; range_len <= one chunk, the bytes in front of the range are its window).  search = 0: the up-front kernels
-// (k_match_shallow / k_match_deep), with the on-demand path switched off for the call.  search = 1: the on-demand search
-// (k_rank_sig + deep_best_warp) at every position of the range; 0 is returned where that path does not run (depth < 64, or a
-// chunk that needs more than one sort batch).
+// test hook (the hash-chain parse: quality 5..9, and 10 / 11 with B200_OPT_Q9_5): best[] of the match stage for the range
+// [range_start, range_start + range_len) of an n-byte buffer (host in, host out; range_len <= one chunk, the bytes in front of the
+// range are its window).  search = 0: the up-front kernels (k_match_shallow / k_match_deep), with the on-demand path switched off
+// for the call.  search = 1: the on-demand search (k_rank_sig + deep_best_warp) at every position of the range; 0 is returned
+// where that path does not run (depth < 64, or a chunk that needs more than one sort batch).
 int b200_stage_match(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n, size_t range_start,
                      size_t range_len, int search, uint32_t* best_out) {
   if (!e || !e->ok || n == 0 || n >= 0xFFFFF000ull || range_len == 0 || range_len > kChunk || range_start > n - range_len) return 0;
-  if (b200_effective_quality(quality) >= 10 || (search != 0 && search != 1)) return 0;
+  if (search != 0 && search != 1) return 0;
   if (cudaSetDevice(e->device) != cudaSuccess) return 0;
   if (!size_hint) size_hint = n;
+  EncParams P;
+  e->fill_params(&P, quality, lgwin, size_hint);
+  if (P.zopfli) return 0;
   if (search) {
-    EncParams P;
-    e->fill_params(&P, quality, lgwin, size_hint);
     const uint64_t payload_max = kBatchMax - (1ull << P.lgwin) - 4096;
     if (P.depth < 64 || range_len > payload_max) return 0;
     if (!e->d_probe.ensure(range_len * 4)) return 0;
@@ -1088,10 +1102,13 @@ int b200_stage_match_slabs(B200Encoder* e, uint32_t* cursors, uint32_t* sizes, u
   return (int)ns;
 }
 
-// test hook (quality >= 10): matches per position, per-unit results and raw commands of an n-byte buffer (n <= one chunk)
+// test hook (the shortest-path parse): matches per position, per-unit results and raw commands of an n-byte buffer (n <= one chunk)
 int b200_stage_hq(B200Encoder* e, int quality, int lgwin, const uint8_t* in, size_t n, uint8_t* hqn, uint32_t* hqm, uint32_t* units,
                   uint32_t* raw) {
-  if (!e || !e->ok || n == 0 || n > kChunk || quality < 10) return 0;
+  if (!e || !e->ok || n == 0 || n > kChunk) return 0;
+  EncParams P;
+  e->fill_params(&P, quality, lgwin, n);
+  if (!P.zopfli) return 0;
   if (cudaSetDevice(e->device) != cudaSuccess) return 0;
   size_t got = 0;
   if (!compress_range_impl(e, quality, lgwin, n, in, n, 0, n, true, true, false, nullptr, b200_max_compressed_size(n) + 64, &got, 0, true)) {
@@ -1132,12 +1149,12 @@ int b200_stage_sort(B200Encoder* e, int quality, int lgwin, const uint8_t* in, s
   return ok && cudaMemcpy(sorted_out, S.b, n * 4, cudaMemcpyDeviceToHost) == cudaSuccess;
 }
 
-// parse unit the quality >= 10 path uses for this size hint with the encoder's current options (sizes the b200_stage_hq buffers)
+// parse unit the shortest-path parse uses for this size hint with the encoder's current options (sizes the b200_stage_hq buffers)
 uint32_t b200_hq_unit(B200Encoder* e, int quality, uint64_t size_hint) {
-  if (!e || quality < 10) return 0;
+  if (!e) return 0;
   EncParams P;
   e->fill_params(&P, quality, 22, size_hint);
-  return P.unit;
+  return P.zopfli ? P.unit : 0;
 }
 
 }  // extern "C"

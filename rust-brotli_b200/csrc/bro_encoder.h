@@ -6,7 +6,8 @@
 extern "C" {
 #endif
 typedef struct B200Encoder B200Encoder;
-enum { B200_OPT_CTX_MODEL = 6, B200_OPT_TIMING = 7, B200_OPT_LANES = 8, B200_OPT_DICT = 9, B200_OPT_HQ_SPLIT = 12, B200_OPT_HQ_UNIT = 13, B200_OPT_ONDEMAND = 15, B200_OPT_HQ_LEVELS = 16 };
+enum { B200_OPT_CTX_MODEL = 6, B200_OPT_TIMING = 7, B200_OPT_LANES = 8, B200_OPT_DICT = 9, B200_OPT_HQ_SPLIT = 12, B200_OPT_HQ_UNIT = 13, B200_OPT_ONDEMAND = 15, B200_OPT_HQ_LEVELS = 16,
+       B200_OPT_Q9_5 = 17 /* BROTLI_PARAM_Q9_5: quality 10 / 11 run the hash-chain parse under their metablock builder */ };
 /* stage timing slots of b200_encoder_last_timings */
 enum { B200_ST_SORT = 0, B200_ST_MATCH = 1, B200_ST_PARSE = 2, B200_ST_FINALIZE = 3, B200_ST_SPLIT = 4, B200_ST_HEADER = 5,
        B200_ST_EMIT = 6, B200_NUM_STAGES = 7 };
@@ -35,10 +36,10 @@ typedef struct B200Prologue {
 } B200Prologue;
 /* b200_encoder_compress_range_async behind a prologue: the range's first metablock starts at byte pro->len (pro may be NULL), and
  * trailer >= 0 appends that byte behind the range's byte-aligned end.  The prologue's n2 data bytes are the input bytes right in
- * front of range_start.  ctx_model / use_dict apply to this call only. */
+ * front of range_start.  ctx_model / use_dict / q9_5 apply to this call only (-1: the encoder's option). */
 int b200_encoder_compress_framed_async(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, int ctx_model, int use_dict,
-                                       const uint8_t* in, size_t n, size_t range_start, size_t range_len, int first, int last,
-                                       int byte_align, const B200Prologue* pro, int trailer, uint8_t* out, size_t out_cap,
+                                       int q9_5, const uint8_t* in, size_t n, size_t range_start, size_t range_len, int first,
+                                       int last, int byte_align, const B200Prologue* pro, int trailer, uint8_t* out, size_t out_cap,
                                        uint64_t* out_size, void* stream);
 int b200_encoder_last_timings(B200Encoder* e, float* ms /* [B200_NUM_STAGES] */, uint32_t* launches);
 int b200_stage_match(B200Encoder* e, int quality, int lgwin, uint64_t size_hint, const uint8_t* in, size_t n, size_t range_start,

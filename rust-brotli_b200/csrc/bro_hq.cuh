@@ -620,31 +620,40 @@ BRO_HD uint32_t hq_default_unit(int quality, uint32_t size_hint) {
   return quality >= 11 ? 16384u : 8192u;
 }
 
-// Default parameters of a (quality, lgwin, size hint) configuration, shared by the device encoder and its CPU model.  P->n and
-// P->abs_base are left 0: they describe the range being compressed.  size_hint = 0 means unknown.
-inline void default_enc_params(EncParams* P, int quality, int lgwin, uint32_t size_hint) {
+// Default parameters of a (quality, lgwin, size hint, Q9_5) configuration, shared by the device encoder and its CPU model.  P->n
+// and P->abs_base are left 0: they describe the range being compressed.  size_hint = 0 means unknown.
+//
+// Q9_5 ("quality 9.5", BROTLI_PARAM_Q9_5) keeps quality 10 / 11 from choosing H10, so the parse is the hash-chain greedy / lazy
+// one (the reference picks the parse from the hasher, backward_references/mod.rs:2553-2780) while everything after the parse --
+// context mode, block split, clustering, distance parameters -- follows the quality.  At every quality it also lowers the size
+// hint above which H6 is chosen from 4 MiB to 1 MiB.
+inline void default_enc_params(EncParams* P, int quality, int lgwin, uint32_t size_hint, int q9_5 = 0) {
   *P = EncParams{};
   quality = effective_quality(quality);
   lgwin = lgwin < 10 ? 10 : (lgwin > 24 ? 24 : lgwin);
   P->quality = quality;
   P->lgwin = lgwin;
   P->size_hint = size_hint;
+  P->zopfli = quality >= 10 && !q9_5;
+  P->hq_meta = quality >= 10;
+  const int block_bits = quality - 1 < 9 ? quality - 1 : 9;
+  const uint32_t h6_hint = q9_5 ? (1u << 20) : (1u << 22);
   // ChooseHasher, encode.rs:834-893 (H40-42 are not implemented there and fall back to H6 with default params)
-  if (quality >= 10) { P->hash_type = 5; P->key_bits = 15; P->hash_len = 4; P->depth = 256; P->n_last = 16; }  // bucket lists for k_match_all (with the long-prefix levels on, 64..1024 give the same size +-0.02 %)
-  else if (quality == 9) { P->hash_type = 9; P->key_bits = 15; P->hash_len = 4; P->depth = 256; P->n_last = 16; }
+  if (P->zopfli) { P->hash_type = 5; P->key_bits = 15; P->hash_len = 4; P->depth = 256; P->n_last = 16; }  // bucket lists for k_match_all (with the long-prefix levels on, 64..1024 give the same size +-0.02 %)
+  else if (quality == 9 || quality == 10) { P->hash_type = 9; P->key_bits = 15; P->hash_len = 4; P->depth = 256; P->n_last = 16; }
   else if (lgwin <= 16) { P->hash_type = 6; P->key_bits = 15; P->hash_len = 5; P->depth = 256; P->n_last = 16; }
-  else if (size_hint > (1u << 22) && lgwin >= 19) {
-    P->hash_type = 6; P->key_bits = 15; P->hash_len = 5; P->depth = 1 << (quality - 1);
+  else if (size_hint > h6_hint && lgwin >= 19) {
+    P->hash_type = 6; P->key_bits = 15; P->hash_len = 5; P->depth = 1 << block_bits;
     P->n_last = quality < 7 ? 4 : quality < 9 ? 10 : 16;
   } else {
     P->hash_type = 5; P->key_bits = (quality < 7 && size_hint <= (1u << 20)) ? 14 : 15; P->hash_len = 4;
-    P->depth = 1 << (quality - 1);
+    P->depth = 1 << block_bits;
     P->n_last = quality < 7 ? 4 : quality < 9 ? 10 : 16;
   }
   P->lcap = 64;
   P->unit = 4096;
   P->mb_units = 1024;  // 4 MiB metablocks
-  if (quality >= 10) {  // same metablock span, larger parse units
+  if (P->zopfli) {  // same metablock span, larger parse units
     P->lcap = HQ_LCAP;
     P->unit = hq_default_unit(quality, size_hint);
     P->mb_units = (4u << 20) / P->unit;
@@ -653,7 +662,7 @@ inline void default_enc_params(EncParams* P, int quality, int lgwin, uint32_t si
   P->ctx_model = 1;
   P->use_dict = 1;
   P->hq_split = 1;
-  P->hq_levels = quality >= 10 ? HQ_MAX_LEVELS : 0;
+  P->hq_levels = P->zopfli ? HQ_MAX_LEVELS : 0;
 }
 
 // Quality 11 runs the shortest path twice, the second time with costs taken from the commands of the first pass

@@ -685,14 +685,28 @@ __global__ void __launch_bounds__(MATCH_THREADS) k_match_shallow(MatchArgs a, Be
   match_store(a, st, active, p, outv);
 }
 
-// Deep buckets (depth 64..256: q7..q9 and lgwin <= 16).  With one position per lane the survivors of the 4-byte filter are
-// evaluated by a few active lanes on average, so here the (position,
+// Candidate key of the deep searches: score << 16 | (IMAX - candidate index) << LB | len, so that a maximum is "highest score,
+// nearest on ties".  Scores stay below 2^16.  Up to 256 candidates the index takes 8 bits and the length 8; a 512-deep bucket
+// (quality 11 with Q9_5) takes a 9-bit index and leaves 7 bits to the length, which the match cap (lcap = 64) fits.
+template <int DEPTH>
+struct DeepKey {
+  static_assert(DEPTH <= 512, "candidate index wider than 9 bits");
+  static constexpr uint32_t LB = DEPTH > 256 ? 7u : 8u;
+  static constexpr uint32_t IMAX = (1u << (16u - LB)) - 1u;
+  static constexpr uint32_t LMASK = (1u << LB) - 1u;
+  static __device__ __forceinline__ uint32_t make(uint32_t score, uint32_t idx, uint32_t len) { return (score << 16) | ((IMAX - idx) << LB) | len; }
+  static __device__ __forceinline__ uint32_t index(uint32_t k) { return IMAX - ((k >> LB) & IMAX); }
+};
+
+// Deep buckets (depth 64..512: q7..q9, lgwin <= 16 and quality 11 with Q9_5).  With one position per lane the survivors of the
+// 4-byte filter are evaluated by a few active lanes on average, so here the (position,
 // candidate) pairs of a whole warp are compacted and evaluated 32 at a time; results meet in a per-position atomicMax on
-// score << 16 | (255 - candidate index) << 8 | len.  "Highest score, nearest on ties" is exactly what the sequential
+// DeepKey.  "Highest score, nearest on ties" is exactly what the sequential
 // newest-first walk with strict improvement computes.  The "must be strictly longer" pre-filter uses the best of the
 // *previous* groups only (all nearer), which keeps it exact.
 template <int DEPTH>
 __global__ void __launch_bounds__(MATCH_THREADS) k_match_deep(MatchArgs a) {
+  using K = DeepKey<DEPTH>;
   extern __shared__ __align__(16) uint32_t smem[];
   constexpr uint32_t E = MATCH_THREADS + (uint32_t)DEPTH;
   uint32_t* s_pos = smem;
@@ -809,14 +823,14 @@ __global__ void __launch_bounds__(MATCH_THREADS) k_match_deep(MatchArgs a) {
       }
       if (len > emaxl) len = emaxl;
       const uint32_t score = score_regular(a.hash_type, len, backward);
-      atomicMax(&s_bestk[wid][ln], (score << 16) | ((255u - (cbase + c)) << 8) | len);
+      atomicMax(&s_bestk[wid][ln], K::make(score, cbase + c, len));
     }
     __syncwarp();
     if (!done) {
       const uint32_t bk = s_bestk[wid][lane];
       if (bk != kNone) {
-        s_snap[wid][lane] = bk & 0xFFu;
-        if ((bk & 0xFFu) == maxl) done = true;  // a full-length match: nothing farther can beat it
+        s_snap[wid][lane] = bk & K::LMASK;
+        if ((bk & K::LMASK) == maxl) done = true;  // a full-length match: nothing farther can beat it
       }
       if ((s_far[wid] >> lane) & 1u) done = true;  // candidates beyond the window: all older ones too
     }
@@ -826,8 +840,8 @@ __global__ void __launch_bounds__(MATCH_THREADS) k_match_deep(MatchArgs a) {
     const uint32_t bk = s_bestk[wid][lane];
     uint32_t r = 0;
     if (bk != kNone) {
-      const uint32_t cc = 255u - ((bk >> 8) & 0xFFu);
-      r = ((prel - s_pos[i - 1u - cc]) << 8) | (bk & 0xFFu);
+      const uint32_t cc = K::index(bk);
+      r = ((prel - s_pos[i - 1u - cc]) << 8) | (bk & K::LMASK);
     } else if (a.use_dict && a.n - p >= 8) {
       r = dict_candidate_dev(a.dict, a.hash_type, s_d0[i], s_d1[i], s_d2[i], s_d3[i], a.data + p, a.n - p, bmin(p, a.max_backward));
     }
@@ -1201,8 +1215,12 @@ __global__ void __launch_bounds__(256) k_rank_sig(MatchArgs a, uint32_t* sig) {
   if (pos >= a.payload_begin) a.best[a.origin + pos] = j;
 }
 
+// Words of a warp's survivor list (s_back): every candidate of a bucket may survive the signature filter.
+template <int DEPTH>
+struct DeepSurvivors { static constexpr int N = DEPTH > 256 ? DEPTH : 256; };
+
 // best[p] of k_match_deep for the absolute position p, computed by the whole warp (result uniform).  r = rank of p in the sorted
-// list, s_back = 256 words of shared memory owned by this warp.  A walk is a chain of dependent positions, so what counts is the
+// list, s_back = DeepSurvivors<DEPTH>::N words of shared memory owned by this warp.  A walk is a chain of dependent positions, so what counts is the
 // number of memory round trips per position:
 //   1. positions and signatures of all DEPTH candidates in one go (lane l: candidates l, l + 32, ..; coalesced), bucket / window
 //      end by ballots; the distances of the candidates whose signature agrees are compacted into s_back, nearest first,
@@ -1285,16 +1303,16 @@ __device__ __forceinline__ uint32_t deep_best_warp(const DeepArgs& A, uint32_t p
         }
         if (len) {
           len = bmin(len, maxl);
-          cand = (score_regular(a.hash_type, len, backward) << 16) | ((255u - sidx) << 8) | len;
+          cand = DeepKey<DEPTH>::make(score_regular(a.hash_type, len, backward), sidx, len);
         }
       }
     }
     const uint32_t wmax = __reduce_max_sync(FULL, cand);
-    if (wmax > bestk) { bestk = wmax; bl = wmax & 0xFFu; }
+    if (wmax > bestk) { bestk = wmax; bl = wmax & DeepKey<DEPTH>::LMASK; }
     if (bestk != kNone && bl == maxl) break;
   }
   uint32_t res = 0;
-  if (bestk != kNone) res = (s_back[255u - ((bestk >> 8) & 0xFFu)] << 8) | (bestk & 0xFFu);
+  if (bestk != kNone) res = (s_back[DeepKey<DEPTH>::index(bestk)] << 8) | (bestk & DeepKey<DEPTH>::LMASK);
   else if (a.use_dict) {
     const uint64_t c16 = ldu64(cur + 8);
     res = dict_candidate_dev(a.dict, a.hash_type, (uint32_t)c8, (uint32_t)(c8 >> 32), (uint32_t)c16, (uint32_t)(c16 >> 32), cur, a.n - p, mbk);
@@ -1307,7 +1325,7 @@ __device__ __forceinline__ uint32_t deep_best_warp(const DeepArgs& A, uint32_t p
 // out[len].  Launched right after k_rank_sig (while the ranks, signatures and sorted list are intact) only when a stage hook asks.
 template <int DEPTH>
 __global__ void __launch_bounds__(256) k_od_probe(DeepArgs A, uint32_t start, uint32_t len, uint32_t* out) {
-  __shared__ uint32_t s_back_all[8][256];
+  __shared__ uint32_t s_back_all[8][DeepSurvivors<DEPTH>::N];
   const uint32_t w = blockIdx.x * 8u + (threadIdx.x >> 5);
   if (w >= len) return;
   const uint32_t p = start + w;
@@ -1356,8 +1374,10 @@ __device__ __forceinline__ bool find_match_ondemand(const EncParams& P, const De
   return found;
 }
 
+// (a 512-deep bucket holds 32 candidate registers per lane: at 8 CTAs per SM, i.e. 64 registers, that walk spilled 180 bytes;
+// at 6 it takes 80 registers and spills 64 bytes, about what the 256-deep walk spills at 8)
 template <int NL, int DEPTH>
-__global__ void __launch_bounds__(PARSE_WARPS * 32, 8) k_parse_ondemand(Workspace W, DeepArgs A) {
+__global__ void __launch_bounds__(PARSE_WARPS * 32, DEPTH > 256 ? 6 : 8) k_parse_ondemand(Workspace W, DeepArgs A) {
   const uint32_t u = blockIdx.x * PARSE_WARPS + (threadIdx.x >> 5);
   if (u >= W.num_units) return;
   const EncParams& P = W.P;
@@ -1367,7 +1387,7 @@ __global__ void __launch_bounds__(PARSE_WARPS * 32, 8) k_parse_ondemand(Workspac
   int32_t dc[4] = {0x3fffffff, 0x3fffffff, 0x3fffffff, 0x3fffffff};
   const bool warm = (u % P.mb_units) != 0 && s >= BRO_WARMUP_BYTES;
   RawCmd* const out = W.raw + (size_t)u * (P.unit / 2 + 1);
-  __shared__ uint32_t s_back_all[PARSE_WARPS][256];
+  __shared__ uint32_t s_back_all[PARSE_WARPS][DeepSurvivors<DEPTH>::N];
   uint32_t* const s_back = s_back_all[threadIdx.x >> 5];
   const uint32_t FULL = 0xffffffffu;
   const uint32_t lane = threadIdx.x & 31;
@@ -1733,7 +1753,7 @@ __global__ void __launch_bounds__(256) k_ctx_decide(Workspace W) {
   for (uint32_t i = threadIdx.x; i < sizeof(CtxSampleHist) / 4; i += blockDim.x) raw[i] = 0;
   __syncthreads();
   const EncParams& P = W.P;
-  if (P.quality >= 10 && P.hq_split) {  // ChooseContextMode (encode.rs:1357-1377), decided on the first 64 KiB
+  if (P.hq_meta && P.hq_split) {  // ChooseContextMode (encode.rs:1357-1377), decided on the first 64 KiB
     if (threadIdx.x == 0) mb.ctx_map_id = hq_is_mostly_utf8(W.data + mb.start, bmin(mb.len, 65536u)) ? CTXMAP_FULL_UTF8 : CTXMAP_FULL_SIGNED;
     return;
   }

@@ -45,8 +45,12 @@ struct EncParams {
   uint32_t size_hint;
   int ctx_model;      // literal context modelling on/off
   int use_dict;       // static-dictionary matches on/off
-  int hq_split;       // quality >= 10: 1 = BrotliSplitBlock + clustered context maps (default), 0 = the greedy splitter of q5..q9
-  int hq_levels;      // quality >= 10: number of long-prefix candidate levels (8, 16, 32 bytes) on top of the 4-byte buckets: 0..3
+  int hq_split;       // with hq_meta: 1 = BrotliSplitBlock + clustered context maps (default), 0 = the greedy splitter of q5..q9
+  int hq_levels;      // with zopfli: number of long-prefix candidate levels (8, 16, 32 bytes) on top of the 4-byte buckets: 0..3
+  // The two families a configuration runs, derived from (quality, Q9_5) by default_enc_params and read everywhere else:
+  int zopfli;         // parse: 1 = all matches + shortest path (H10, q10 / q11), 0 = bucket match + greedy / lazy (q5..q9, 9.5)
+  int hq_meta;        // metablock builder: 1 = ChooseContextMode, BrotliSplitBlock, clustered context maps and the NPOSTFIX /
+                      //   NDIRECT search (quality 10 / 11, with or without Q9_5), 0 = the greedy splitter of q5..q9
 };
 
 // ---- scores ----

@@ -42,6 +42,7 @@ pub mod param {
     pub const DISABLE_LITERAL_CONTEXT_MODELING: u32 = 4;
     pub const SIZE_HINT: u32 = 5;
     pub const LARGE_WINDOW: u32 = 6;
+    pub const Q9_5: u32 = 150;
     pub const CATABLE: u32 = 167;
     pub const APPENDABLE: u32 = 168;
     pub const MAGIC_NUMBER: u32 = 169;

@@ -31,6 +31,8 @@ pub struct BrotliEncoderParams {
     pub byte_align: bool,
     pub bare_stream: bool,
     pub use_dictionary: bool,
+    /// "quality 9.5": with quality 10 / 11, the hash-chain parse under the quality 10 / 11 metablock builder
+    pub q9_5: bool,
 }
 
 impl Default for BrotliEncoderParams {
@@ -38,7 +40,7 @@ impl Default for BrotliEncoderParams {
         // encode.rs:318-357
         BrotliEncoderParams { mode: 0, quality: 11, lgwin: 22, lgblock: 0, size_hint: 0, disable_literal_context_modeling: 0,
                               catable: false, appendable: false, magic_number: false, byte_align: false, bare_stream: false,
-                              use_dictionary: true }
+                              use_dictionary: true, q9_5: false }
     }
 }
 
@@ -50,6 +52,7 @@ impl BrotliEncoderParams {
         if self.size_hint != 0 { kv.push((SIZE_HINT, std::cmp::min(self.size_hint, u32::MAX as usize) as u32)); }
         if self.disable_literal_context_modeling != 0 { kv.push((DISABLE_LITERAL_CONTEXT_MODELING, 1)); }
         if !self.use_dictionary { kv.push((NO_DICTIONARY, 1)); }
+        if self.q9_5 { kv.push((Q9_5, 1)); }
         for (k, on) in [(CATABLE, self.catable), (APPENDABLE, self.appendable), (MAGIC_NUMBER, self.magic_number),
                         (BYTE_ALIGN, self.byte_align), (BARE_STREAM, self.bare_stream)].iter() {
             if *on { kv.push((*k, 1)); }

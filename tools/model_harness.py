@@ -6,7 +6,7 @@ _ROOT = os.path.dirname(_HERE)
 class EncParams(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int) for n in ("quality", "lgwin", "hash_type", "key_bits", "hash_len", "depth", "n_last")] + \
                [(n, ctypes.c_uint32) for n in ("lcap", "unit", "mb_units", "max_backward", "n", "abs_base", "size_hint")] + \
-               [(n, ctypes.c_int) for n in ("ctx_model", "use_dict", "hq_split", "hq_levels")]
+               [(n, ctypes.c_int) for n in ("ctx_model", "use_dict", "hq_split", "hq_levels", "zopfli", "hq_meta")]
 
 class ModelStats(ctypes.Structure):
     _fields_ = [(n, ctypes.c_uint64) for n in ("num_metablocks", "num_raw_metablocks", "num_commands", "num_literals", "header_bits", "body_bits")] + \
@@ -30,11 +30,13 @@ class Model:
         self.lib.gpu_model_compress.restype = ctypes.c_size_t
         self.lib.gpu_model_compress.argtypes = [ctypes.POINTER(EncParams), ctypes.c_char_p, ctypes.c_char_p, ctypes.c_size_t,
                                                 ctypes.POINTER(ModelStats), ctypes.c_void_p]
-        self.lib.gpu_model_default_params.argtypes = [ctypes.POINTER(EncParams), ctypes.c_int, ctypes.c_int, ctypes.c_uint32, ctypes.c_uint32]
+        self.lib.gpu_model_default_params.argtypes = [ctypes.POINTER(EncParams), ctypes.c_int, ctypes.c_int, ctypes.c_uint32, ctypes.c_uint32,
+                                                      ctypes.c_int]
         self.lib.gpu_model_debug_hq.argtypes = [ctypes.c_void_p] * 4
-    def params(self, q, lgwin, n, size_hint=0, **kw):
+    def params(self, q, lgwin, n, size_hint=0, q9_5=False, **kw):
+        """Default parameters of a configuration (q9_5: BROTLI_PARAM_Q9_5), then the fields of kw."""
         p = EncParams()
-        self.lib.gpu_model_default_params(ctypes.byref(p), q, lgwin, n, size_hint)
+        self.lib.gpu_model_default_params(ctypes.byref(p), q, lgwin, n, size_hint, int(bool(q9_5)))
         for k, v in kw.items(): setattr(p, k, v)
         return p
     def compress_range(self, data, start, length, q, lgwin, first, last, byte_align, size_hint=0, best_out=None, **kw):
@@ -60,11 +62,11 @@ class Model:
         return out.raw[:n], st
 
     def stage_hq(self, data, q, lgwin, **kw):
-        """Quality 10 / 11 stage results of a one-chunk input, laid out as DeviceEncoder.stage_hq returns them:
+        """Shortest-path parse (quality 10 / 11 without Q9_5) stage results of a one-chunk input, laid out as DeviceEncoder.stage_hq returns them:
         (hqn, hqm, units, raw, unit)."""
         import numpy as np
         n = len(data)
-        if not 0 < n <= 24 << 20 or q < 10:
+        if not 0 < n <= 24 << 20 or not self.params(q, lgwin, n, 0, **kw).zopfli:
             raise ValueError("stage_hq covers one chunk (1 .. 24 MiB) at quality >= 10")
         unit = self.params(q, lgwin, n, 0, **kw).unit
         nu = (n + unit - 1) // unit
