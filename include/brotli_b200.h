@@ -316,6 +316,10 @@ int b200_stage_match(B200Encoder* e, int quality, int lgwin, uint64_t size_hint,
  * match kernel claimed in slab s and sizes[s] = records slab s must receive (s < cap).  Returns the number of slabs, 0 when
  * the last call did not stage best[]. */
 int b200_stage_match_slabs(B200Encoder* e, uint32_t* cursors, uint32_t* sizes, uint32_t cap);
+/* the same for the tiles of 2^13 positions of each batch's payload that the placement fills after the slabs: cursors[t] = records
+ * claimed in tile t of the last batch, sizes[t] = records tile t must receive (t < cap).  Returns the number of tiles, 0 when the
+ * last call did not stage best[]. */
+int b200_stage_match_tiles(B200Encoder* e, uint32_t* cursors, uint32_t* sizes, uint32_t cap);
 /* stage hook of quality 10 / 11 (n <= one chunk): matches per position hqn[n], hqm[n][16][2] (distance, length word); per parse
  * unit ncmd, tail, ncopy as units[3][nu]; raw commands raw[nu][unit / 2 + 1][3].  b200_hq_unit gives the unit for size_hint n. */
 int b200_stage_hq(B200Encoder* e, int quality, int lgwin, const uint8_t* in, size_t n, uint8_t* hqn, uint32_t* hqm, uint32_t* units,

@@ -68,6 +68,8 @@ def lib():
         L.b200_stage_match.restype = ctypes.c_int
         L.b200_stage_match_slabs.argtypes = [vp, vp, vp, ctypes.c_uint32]
         L.b200_stage_match_slabs.restype = ctypes.c_int
+        L.b200_stage_match_tiles.argtypes = [vp, vp, vp, ctypes.c_uint32]
+        L.b200_stage_match_tiles.restype = ctypes.c_int
         L.b200_stage_hq.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp, sz, vp, vp, vp, vp]
         L.b200_stage_hq.restype = ctypes.c_int
         L.b200_hq_unit.argtypes = [vp, ctypes.c_int, ctypes.c_uint64]
@@ -221,6 +223,19 @@ class DeviceEncoder:
         if ns <= 0 or ns > 64:
             raise RuntimeError("b200_stage_match_slabs failed")
         return cursors[:ns], sizes[:ns]
+
+    def stage_match_tiles(self):
+        """The same as stage_match_slabs for the tiles of 2^13 positions that the placement fills after the slabs: (cursors,
+        sizes) with one entry per tile of the last sort batch."""
+        import numpy as np
+        nt = self._L.b200_stage_match_tiles(self._h, None, None, 0)
+        if nt <= 0:
+            raise RuntimeError("b200_stage_match_tiles failed")
+        cursors = np.zeros(nt, dtype=np.uint32)
+        sizes = np.zeros(nt, dtype=np.uint32)
+        if self._L.b200_stage_match_tiles(self._h, cursors.ctypes.data, sizes.ctypes.data, nt) != nt:
+            raise RuntimeError("b200_stage_match_tiles failed")
+        return cursors, sizes
 
     def stage_hq(self, data: bytes, quality: int, lgwin: int):
         """Quality 10 / 11 stage results of one chunk: (hqn[n] u8, hqm[n][16][2] u32 (dist, lc), units[3][nu] u32 (ncmd, tail,

@@ -99,7 +99,8 @@ struct Lane {
   DevBuf arena;     // every region of the chunk workspace (layout_chunk)
   Workspace W{};    // the last chunk's workspace: the stage hooks read their results through it
   const uint32_t* slab_cursor = nullptr;  // the last chunk's last sort batch, when its best[] went through match_store:
-  uint32_t slab_payload = 0;              //   its slab cursors and payload size (b200_stage_match_slabs)
+  const uint32_t* tile_cursor = nullptr;  //   its slab and tile cursors and payload size (b200_stage_match_slabs,
+  uint32_t slab_payload = 0;              //   b200_stage_match_tiles)
   EventPool marks;  // timing marks: (event, stage that starts there); -1 ends the last stage
   std::vector<int> mark_stage;
   void release() {
@@ -126,14 +127,16 @@ struct Carve {
 };
 
 struct SortBufs {
-  uint32_t *a, *b;  // ping-pong of the sort passes; the sorted positions land in b
+  uint32_t *a, *b;  // ping-pong of the sort passes, the two halves of one region; the sorted positions land in b
   uint32_t* state;  // digit counts, tile counters and look-back words
 };
-// sort regions for batches of up to nb positions
+// sort regions for batches of up to nb positions.  Once the match kernel has read the sorted list, the whole ping-pong region
+// (8 · nb bytes or more) is free: k_best_bin uses it as the tile-major buffer of a batch's payload (at most nb records of 8 B).
 SortBufs layout_sort(Carve& a, uint32_t nb) {
   SortBufs s;
-  s.a = a.take<uint32_t>((size_t)nb + 16);  // (+ 64 bytes)
-  s.b = a.take<uint32_t>((size_t)nb + 16);
+  const size_t half = ((size_t)nb + 16 + 63) & ~(size_t)63;  // (+ 64 bytes; b stays 256-byte aligned)
+  s.a = a.take<uint32_t>(2 * half);
+  s.b = s.a ? s.a + half : nullptr;
   s.state = a.take<uint32_t>(sort_state_words((nb + SORT_TILE - 1) / SORT_TILE));
   return s;
 }
@@ -185,7 +188,7 @@ void layout_hq_split(Carve& a, const EncParams& P, const Workspace& W, BsWs* B, 
 
 struct ChunkBufs {  // the regions of a chunk that Workspace does not point to
   SortBufs sort;
-  uint2* stage;         // bucket depth 16 / 32: best[] records of a sort batch, slab-major (match_store)
+  uint2* stage;         // bucket depth 16 / 32: best[] records of a sort batch, slab-major (match_store); tile-major in sort.a
   ZopfliArgs za;        // zopfli
   BsWs bs;              // hq_meta with hq_split
   CmWs cm;              //   "
@@ -368,6 +371,7 @@ struct B200Encoder {
     CUDA_OK(cudaMemcpy(d_dict_tr.p, kDictTransforms, sizeof(kDictTransforms), cudaMemcpyHostToDevice));
     CUDA_OK(cudaDeviceSetLimit(cudaLimitStackSize, 4096));
     CUDA_OK(cudaFuncSetAttribute(k_split_greedy, cudaFuncAttributeMaxDynamicSharedMemorySize, SPLIT_SMEM_WORDS * 4));
+    CUDA_OK(cudaFuncSetAttribute(k_best_bin, cudaFuncAttributeMaxDynamicSharedMemorySize, BEST_BIN_SPAN * 8));
     for (int i = 0; i < B200_NUM_STAGES; ++i) stage_ms[i] = 0;
     ok = true;
     return true;
@@ -592,7 +596,7 @@ struct B200Encoder {
     const bool od = od_shape && (ondemand > 1 || (ondemand == 1 && P.depth >= 128 && range_len >= ((uint32_t)4 << 20)));
     DeepArgs da;
     memset(&da, 0, sizeof(da));
-    L.slab_cursor = nullptr;
+    L.slab_cursor = L.tile_cursor = nullptr;
     for (uint64_t b0 = range_start; b0 < (uint64_t)range_start + range_len; b0 += payload_max) {
       const uint32_t b1 = (uint32_t)std::min<uint64_t>((uint64_t)range_start + range_len, b0 + payload_max);
       uint32_t origin = b0 > window ? (uint32_t)b0 - window : 0u;
@@ -663,12 +667,18 @@ struct B200Encoder {
           case 512: k_match_deep<512><<<mgrid, MATCH_THREADS, smem, stream>>>(ma); break;
           default: fprintf(stderr, "[brotli_b200] unsupported bucket depth %d\n", P.depth); return false;
         }
-        if (P.depth <= 32) {  // k_match_shallow left one record per payload position in X.stage
+        if (P.depth <= 32) {  // k_match_shallow left one record per payload position in X.stage; the sorted list is dead now
           const uint32_t payload = b1 - (uint32_t)b0;
-          k_best_place<<<(payload + 255) / 256, 256, 0, stream>>>(X.stage, payload, ma.best);
+          uint2* tiles = reinterpret_cast<uint2*>(X.sort.a);
+          uint32_t* tile_cursor = X.sort.state + SORT_ST_BTILE;  // zeroed by run_sort
+          k_best_bin<<<(payload + BEST_BIN_SPAN - 1) / BEST_BIN_SPAN, BEST_BIN_THREADS, BEST_BIN_SPAN * 8, stream>>>(
+              X.stage, payload, (uint32_t)b0, tiles, tile_cursor);
+          k_best_tile<<<(payload + (1u << BEST_TILE_BITS) - 1) >> BEST_TILE_BITS, BEST_TILE_THREADS, 0, stream>>>(
+              tiles, payload, (uint32_t)b0, ma.best);
           L.slab_cursor = bs.slab_cursor;
+          L.tile_cursor = tile_cursor;
           L.slab_payload = payload;
-          launches += 1;
+          launches += 2;
         }
       }
       launches += 1;
@@ -1100,6 +1110,19 @@ int b200_stage_match_slabs(B200Encoder* e, uint32_t* cursors, uint32_t* sizes, u
   if (cudaMemcpy(cursors, L.slab_cursor, (size_t)k * 4, cudaMemcpyDeviceToHost) != cudaSuccess) return 0;
   for (uint32_t s = 0; s < k; ++s) sizes[s] = std::min(1u << BEST_SLAB_BITS, L.slab_payload - (s << BEST_SLAB_BITS));
   return (int)ns;
+}
+
+// test hook: as b200_stage_match_slabs, for the tiles of 2^BEST_TILE_BITS positions that k_best_bin fills: the records it claimed
+// in each tile of the range's last sort batch and the number each tile must receive.  Returns the number of tiles.
+int b200_stage_match_tiles(B200Encoder* e, uint32_t* cursors, uint32_t* sizes, uint32_t cap) {
+  if (!e || !e->ok || cudaSetDevice(e->device) != cudaSuccess) return 0;
+  const Lane& L = e->lanes[0];
+  if (!L.tile_cursor) return 0;
+  const uint32_t nt = (L.slab_payload + (1u << BEST_TILE_BITS) - 1) >> BEST_TILE_BITS;
+  const uint32_t k = std::min(nt, cap);
+  if (k && cudaMemcpy(cursors, L.tile_cursor, (size_t)k * 4, cudaMemcpyDeviceToHost) != cudaSuccess) return 0;
+  for (uint32_t t = 0; t < k; ++t) sizes[t] = std::min(1u << BEST_TILE_BITS, L.slab_payload - (t << BEST_TILE_BITS));
+  return (int)nt;
 }
 
 // test hook (the shortest-path parse): matches per position, per-unit results and raw commands of an n-byte buffer (n <= one chunk)

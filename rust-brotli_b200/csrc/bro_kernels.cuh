@@ -207,7 +207,8 @@ __device__ __forceinline__ void tma_stage_tile(void* smem_dst, const void* gmem_
 #define SORT_ST_DONE 1024   // k_sort_count CTAs that have added their counts
 #define SORT_ST_TILE 1025   // [2] next tile index of each pass
 #define SORT_ST_SLAB 1032   // [BEST_MAX_SLABS] records claimed in each best[] slab by k_match_shallow in the batch (match_store)
-#define SORT_ST_FLAGS 1056  // [2][num_tiles][256] look-back words: flag bits | count
+#define SORT_ST_BTILE 1056  // [BEST_MAX_TILES] records claimed in each best[] tile by k_best_bin in the batch
+#define SORT_ST_FLAGS 5152  // [2][num_tiles][256] look-back words: flag bits | count
 #define SORT_LB_AGG (1u << 30)  // count of the digit in this tile alone
 #define SORT_LB_INC (2u << 30)  // count of the digit in this tile and every tile before it
 #define SORT_LB_VAL 0x3FFFFFFFu
@@ -490,17 +491,31 @@ struct MatchArgs {
   int use_dict;
 };
 
-// best[] of a batch at depth 16 / 32 is written in two steps.  k_match_shallow's positions are in bucket order, so a direct best[p] store puts 4
-// bytes at a random address of the whole payload: every store is a partial 32-byte sector of its own, written back (and
-// fill-read) alone.  Instead the payload [b0, b1) is cut into slabs of 2^BEST_SLAB_BITS positions counted from b0.  Every
-// payload position yields exactly one record, so slab s receives exactly min(2^BEST_SLAB_BITS, b1 - b0 - (s << BEST_SLAB_BITS))
-// records and owns that many 8-byte slots of `stage` from s << BEST_SLAB_BITS on.  match_store bins a CTA's records by slab,
-// claims one contiguous run per slab with one atomic and writes the run; k_best_place then walks `stage` in order, so the live
-// best[] store window is about one slab (8 MB), whose sectors are complete in L2 before they are evicted.  The values placed are
-// the ones a direct store writes; only the order of the records within a slab varies from run to run.
+// best[] of a batch at depth 16 / 32 is written in three steps.  k_match_shallow's positions are in bucket order, so a direct best[p]
+// store puts 4 bytes at a random address of the whole payload: every store is a write request of its own.  Instead the payload
+// [b0, b1) is cut into slabs of 2^BEST_SLAB_BITS positions and those into tiles of 2^BEST_TILE_BITS positions, both counted from
+// b0.  Every payload position yields exactly one record, so slab s receives exactly min(2^BEST_SLAB_BITS, b1 - b0 - (s <<
+// BEST_SLAB_BITS)) records and owns that many 8-byte slots of `stage` from s << BEST_SLAB_BITS on, and tile t likewise owns its
+// size's slots of the tile-major buffer from t << BEST_TILE_BITS on; no count has to be scanned first.
+//   match_store   bins a CTA's records by slab, claims one run per slab with one atomic and writes the run (slab-major `stage`)
+//   k_best_bin    reads BEST_BIN_SPAN records of one slab, reorders them by tile in shared memory, claims one run per tile and
+//                 writes the runs (tile-major buffer; a run is about 32 records at 2^13-position tiles)
+//   k_best_tile   reads one tile's records, places each value in a shared-memory image of the tile's best[] and writes the image
+//                 with 16-byte stores
+// Every global access of the last two is a coalesced stream.  The values placed are the ones a direct store writes; only the
+// order of the records within a slab or a tile varies from run to run.
 #define BEST_SLAB_BITS 21
-#define BEST_MAX_SLABS 16  // kBatchMax >> BEST_SLAB_BITS
-static_assert(SORT_ST_SLAB + BEST_MAX_SLABS <= SORT_ST_FLAGS, "slab cursors overlap the look-back words");
+#define BEST_MAX_SLABS 16                                  // kBatchMax >> BEST_SLAB_BITS
+#define BEST_TILE_BITS 13                                  // a 32 KiB tile of best[]
+#define BEST_MAX_TILES (1u << (25 - BEST_TILE_BITS))       // kBatchMax >> BEST_TILE_BITS
+#define BEST_TILES_PER_SLAB (1u << (BEST_SLAB_BITS - BEST_TILE_BITS))
+#define BEST_BIN_SPAN 8192                                 // records per k_best_bin CTA; divides a slab, so a span lies in one slab
+#define BEST_BIN_THREADS 256
+#define BEST_TILE_THREADS 256
+static_assert(SORT_ST_SLAB + BEST_MAX_SLABS <= SORT_ST_BTILE, "slab cursors overlap the tile cursors");
+static_assert(SORT_ST_BTILE + BEST_MAX_TILES <= SORT_ST_FLAGS, "tile cursors overlap the look-back words");
+static_assert(((1u << BEST_SLAB_BITS) % BEST_BIN_SPAN) == 0 && BEST_BIN_SPAN % BEST_BIN_THREADS == 0, "a span crosses a slab");
+static_assert(BEST_TILE_BITS <= BEST_SLAB_BITS && ((1u << BEST_TILE_BITS) % (4 * BEST_TILE_THREADS)) == 0, "tile shape");
 struct BestStage {
   uint2* stage;           // [payload] (position, value) records, slab-major
   uint32_t* slab_cursor;  // [BEST_MAX_SLABS] records claimed per slab, zeroed with the sort state
@@ -526,12 +541,89 @@ __device__ __forceinline__ void match_store(const MatchArgs& a, const BestStage&
   if (active) st.stage[((size_t)slab << BEST_SLAB_BITS) + s_run[slab] + rank] = make_uint2(p, v);
 }
 
-// best[pos] = value for the `count` records of `stage`, in order (slab after slab)
-__global__ void __launch_bounds__(256) k_best_place(const uint2* __restrict__ stage, uint32_t count, uint32_t* __restrict__ best) {
-  const uint32_t k = blockIdx.x * 256u + threadIdx.x;
-  if (k >= count) return;
-  const uint2 r = __ldcs(&stage[k]);  // read once
-  best[r.x] = r.y;
+// slab-major `stage` -> tile-major `tiles` for the `payload` records of the batch whose payload starts at absolute position b0;
+// one CTA per span of BEST_BIN_SPAN records, dynamic shared memory BEST_BIN_SPAN records, tile_cursor zeroed with the sort state
+__global__ void __launch_bounds__(BEST_BIN_THREADS, 2) k_best_bin(const uint2* __restrict__ stage, uint32_t payload, uint32_t b0,
+                                                                 uint2* __restrict__ tiles, uint32_t* __restrict__ tile_cursor) {
+  constexpr uint32_t ITEMS = BEST_BIN_SPAN / BEST_BIN_THREADS;
+  constexpr uint32_t TPS = BEST_TILES_PER_SLAB;
+  constexpr uint32_t TPT = (TPS + BEST_BIN_THREADS - 1) / BEST_BIN_THREADS;  // tiles per thread in the scan
+  extern __shared__ uint2 s_rec[];                                             // [BEST_BIN_SPAN] the span in tile order
+  __shared__ uint32_t s_cnt[TPS], s_off[TPS], s_run[TPS];
+  __shared__ uint32_t s_warp[BEST_BIN_THREADS / 32];
+  const uint32_t tid = threadIdx.x;
+  const uint32_t k0 = blockIdx.x * BEST_BIN_SPAN;
+  const uint32_t nk = min((uint32_t)BEST_BIN_SPAN, payload - k0);
+  for (uint32_t t = tid; t < TPS; t += BEST_BIN_THREADS) s_cnt[t] = 0;
+  uint2 r[ITEMS];
+#pragma unroll
+  for (uint32_t j = 0; j < ITEMS; ++j) {
+    const uint32_t k = j * BEST_BIN_THREADS + tid;
+    r[j] = k < nk ? __ldcs(&stage[k0 + k]) : make_uint2(0u, 0u);  // read once
+  }
+  __syncthreads();
+  // rank of each record among the span's records of its tile
+  uint32_t rank[ITEMS];
+#pragma unroll
+  for (uint32_t j = 0; j < ITEMS; ++j)
+    if (j * BEST_BIN_THREADS + tid < nk) rank[j] = atomicAdd(&s_cnt[((r[j].x - b0) >> BEST_TILE_BITS) & (TPS - 1)], 1u);
+  __syncthreads();
+  // each tile's first slot in s_rec, and its run in the tile-major buffer
+  uint32_t c[TPT], sum = 0;
+#pragma unroll
+  for (uint32_t q = 0; q < TPT; ++q) {
+    const uint32_t t = tid * TPT + q;
+    c[q] = t < TPS ? s_cnt[t] : 0u;
+    sum += c[q];
+  }
+  uint32_t off = block_excl_scan256(sum, s_warp);
+  const uint32_t tile0 = (k0 >> BEST_SLAB_BITS) * TPS;  // the slab's first tile
+#pragma unroll
+  for (uint32_t q = 0; q < TPT; ++q) {
+    const uint32_t t = tid * TPT + q;
+    if (t < TPS) {
+      s_off[t] = off;
+      if (c[q]) s_run[t] = atomicAdd(&tile_cursor[tile0 + t], c[q]);
+      off += c[q];
+    }
+  }
+  __syncthreads();
+#pragma unroll
+  for (uint32_t j = 0; j < ITEMS; ++j)
+    if (j * BEST_BIN_THREADS + tid < nk) s_rec[s_off[((r[j].x - b0) >> BEST_TILE_BITS) & (TPS - 1)] + rank[j]] = r[j];
+  __syncthreads();
+  // one run per tile, consecutive threads on consecutive slots
+  for (uint32_t i = tid; i < nk; i += BEST_BIN_THREADS) {
+    const uint2 rec = s_rec[i];
+    const uint32_t g = (rec.x - b0) >> BEST_TILE_BITS, t = g & (TPS - 1);
+    tiles[((size_t)g << BEST_TILE_BITS) + s_run[t] + (i - s_off[t])] = rec;
+  }
+}
+
+// tile-major `tiles` -> best[pos] = value (best indexed by absolute position; best + b0 is 16-byte aligned); one CTA per tile
+__global__ void __launch_bounds__(BEST_TILE_THREADS) k_best_tile(const uint2* __restrict__ tiles, uint32_t payload, uint32_t b0,
+                                                                 uint32_t* __restrict__ best) {
+  constexpr uint32_t TILE = 1u << BEST_TILE_BITS, ITEMS = TILE / BEST_TILE_THREADS;
+  __shared__ __align__(16) uint32_t s_img[TILE];
+  const uint32_t tid = threadIdx.x;
+  const uint32_t base = blockIdx.x << BEST_TILE_BITS;  // payload-relative first position of the tile
+  const uint32_t m = min(TILE, payload - base);
+  const uint2* rec = tiles + base;
+  uint2 r[ITEMS];
+#pragma unroll
+  for (uint32_t j = 0; j < ITEMS; ++j) {
+    const uint32_t i = j * BEST_TILE_THREADS + tid;
+    if (i < m) r[j] = __ldcs(&rec[i]);  // read once
+  }
+  const uint32_t pos0 = b0 + base;
+#pragma unroll
+  for (uint32_t j = 0; j < ITEMS; ++j)
+    if (j * BEST_TILE_THREADS + tid < m) s_img[r[j].x - pos0] = r[j].y;
+  __syncthreads();
+  uint4* d4 = reinterpret_cast<uint4*>(best + pos0);
+  const uint4* s4 = reinterpret_cast<const uint4*>(s_img);
+  for (uint32_t i = tid; i < m / 4; i += BEST_TILE_THREADS) d4[i] = s4[i];
+  for (uint32_t i = (m & ~3u) + tid; i < m; i += BEST_TILE_THREADS) best[pos0 + i] = s_img[i];
 }
 
 // dict_candidate() of bro_dict.cuh with the position's first 16 bytes already in registers and 8-byte word compares
